@@ -46,6 +46,8 @@ def lib():
                                         C.c_void_p, C.c_int32, C.c_char_p]
         L.dada2b_test_loop_nw.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, P(_abi.Opts),
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p]
+        L.dada2b_test_screen.argtypes = [C.c_void_p, C.c_uint32, P(_abi.Opts), C.c_double, C.c_uint32, C.c_void_p, C.c_int32, C.c_int32,
+                                         C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p]
         _LIB = L
     return _LIB
 
@@ -71,6 +73,7 @@ class Resident:
         L = lib()
         if len(seqs) == 0:
             raise Dada2bError("Zero input sequences.")                 # Rmain.cpp:55
+        self.nraw = len(seqs)
         try:
             self._pin = _abi.PackedIn(seqs, abundances, priors, None, quals)
         except ValueError as e:
@@ -165,6 +168,26 @@ class Resident:
         if rc:
             raise Dada2bError(eb.value.decode())
         return dict(lam=lam, nsubs=nsubs, handled=handled)
+
+    def test_screen(self, centre, kdist_cutoff=0.42, centre_reads=None, lock=None, rank=0, world=1, max_sms=0, path=0, **opts):
+        """Kernel-level hook (include/dada2b_test.h): one round's k-mer screen of `centre` against the raws of shard (rank, world)
+        -> kind (-1 other rank, 0 shrouded or skipped, 1 gapless, 2 NW), minsum (k_prescreen's, 0xFFFF overflowed, -1 no
+        candidate), counters {align, shroud, gapless, nw}.  `greedy` goes in with the other options; centre_reads defaults to 0."""
+        o = _abi.make_opts(**_normalise_opts(dict(opts)))
+        n = self.nraw
+        lk = None
+        if lock is not None:
+            lk = np.ascontiguousarray(lock, dtype=np.uint8)
+            if len(lk) != n:
+                raise ValueError("lock needs one entry per raw")
+        kind = np.zeros(n, np.int32); minsum = np.zeros(n, np.int32); ctr = np.zeros(4, np.int64)
+        eb = C.create_string_buffer(_abi.ERRLEN)
+        rc = lib().dada2b_test_screen(self._ctx, int(centre), C.byref(o), float(kdist_cutoff), int(centre_reads or 0),
+                                      lk.ctypes.data if lk is not None else None, int(rank), int(world), int(max_sms), int(path),
+                                      kind.ctypes.data, minsum.ctypes.data, ctr.ctypes.data, eb)
+        if rc:
+            raise Dada2bError(eb.value.decode())
+        return dict(kind=kind, minsum=minsum, counters=dict(zip(("align", "shroud", "gapless", "nw"), ctr.tolist())))
 
     def close(self):
         if getattr(self, "_ctx", None) and self._ctx.value:

@@ -15,7 +15,7 @@ def needs_build():
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(os.path.dirname(HERE), "include", f) for f in ("dada2b.h", "dada2b_bimera.h", "dada2b_merge.h", "dada2b_derep.h")]
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(os.path.dirname(HERE), "include", f) for f in ("dada2b.h", "dada2b_test.h", "dada2b_bimera.h", "dada2b_merge.h", "dada2b_derep.h")]
     deps.append(os.path.abspath(__file__))          # FLAGS (target architecture) live here: a library built with other flags is stale
     return any(os.path.getmtime(d) > t for d in deps)
 

@@ -246,6 +246,19 @@ struct dada2b_ctx {
   }
 };
 
+// SMs the dada() path sizes its grids from: the device's count, or fewer under DADA2B_SMS=<n> (test hook: with a small cap,
+// golden-sized inputs give every CTA of the grid-stride kernels several tiles / jobs, as 1e6-unique runs do on all SMs).
+// Every grid is min(work, k * SMs) with a floor of one CTA, so any cap >= 1 is valid.
+static int dada_sms(int device) {
+  int sms = 0; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+  if (const char *e = getenv("DADA2B_SMS")) {
+    const int cap = atoi(e);
+    if (cap < 1) throw Err{"dada2b: DADA2B_SMS must be a positive integer"};
+    sms = std::min(sms, cap);
+  }
+  return sms;
+}
+
 // ------------------------------------------------------------------------------------
 // upload: validation of Rmain.cpp:52-78, raw_new (containers.cpp:19-43) and packing
 // ------------------------------------------------------------------------------------
@@ -264,8 +277,7 @@ static dada2b_ctx *do_upload(const dada2b_in *in, int device, dada2b_ctx *reuse 
     fresh.reset(new dada2b_ctx());
     cx = fresh.get();
     cx->device = device;
-    int sms = 0; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-    cx->num_sms = sms;
+    cx->num_sms = dada_sms(device);
     CK(cudaStreamCreateWithFlags(&cx->stream, cudaStreamNonBlocking));
   }
   DBG("upload: device ready, %d SMs", cx->num_sms);
@@ -425,8 +437,7 @@ dada2b_ctx *ctx_create_device(int device, int nraw, int maxlen, int minlen, cons
     CK(cudaSetDevice(device));
     std::unique_ptr<dada2b_ctx> cx(new dada2b_ctx());
     cx->device = device;
-    int sms = 0; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-    cx->num_sms = sms;
+    cx->num_sms = dada_sms(device);
     CK(cudaStreamCreateWithFlags(&cx->stream, cudaStreamNonBlocking));
     cx->has_quals = true; cx->bad_nt = false; cx->maxq = 0;
     cx->len.resize(nraw); cx->reads.resize(nraw); cx->prior.assign(nraw, 0);
@@ -524,7 +535,10 @@ struct Run {
   unsigned n_ovf = 0;                     // this rank's raws whose repeated-5-mer list overflowed (they alone need the warp-per-pair screen)
   DBuf<unsigned> d_novf;   // dada2b_ctx::upload_gen the k-mer tables were built for
   int nown = 0;
-  bool fallback_only = false;          // DADA2B_FALLBACK (test switch): general kernels only
+  // the shard (raw it * scr_world + scr_rank) and SM count the k-mer screen works with: the context's in a run, the caller's in
+  // the stage hook dada2b_test_screen
+  int scr_rank = 0, scr_world = 1, scr_sms = 1;
+  bool fallback_only = false;         // DADA2B_FALLBACK (test switch): general kernels only
   bool two_phase = false;              // bound pass first, exact lambda for the survivors only (plain gap costs)
   // fused round tail (experimental, DADA2B_FUSED_TAIL=1; dd_round2.cu)
   bool fused_tail = false;               // dd_round2.cu: link + NP passes + final (default); dd_round.cu's split tail otherwise
@@ -627,6 +641,10 @@ struct Run {
   }
   void d2h_pinned(void *h, const void *d, size_t n) { d2h_bytes += (long long)n; CK(cudaMemcpyAsync(h, d, n, cudaMemcpyDeviceToHost, s)); }
 
+  void bind(dada2b_ctx *c, const dada2b_opts *op, int Q) {
+    cx = c; o = op; s = c->stream; in = c->in; nraw = c->in.nraw; ncol = Q;
+    scr_rank = c->rank; scr_world = c->world; scr_sms = c->num_sms;
+  }
   void reset_host();
   void setup_params();
   void alloc_state();
@@ -634,6 +652,7 @@ struct Run {
   void ensure_cs_cap(unsigned long long need);
   void read_ctr() { d2h_pinned(h_ctr.p, ctr.p, CTR_N * 8); sync(); }
   void check_dev_error();
+  void launch_screen(uint32_t c, uint32_t centre_reads, bool greedy, double kdist_cutoff, bool streaming);
   void launch_compare(uint32_t i, double kdist_cutoff);
   void launch_round_tail(int first_pass, int npass);
   void launch_round_tail_inner(int first_pass, int npass);
@@ -777,12 +796,12 @@ void Run::alloc_state() {
   } else { row_mv.free(); row_sub.free(); lane_max = 0; }
   prescreen = P.use_kmers && !fallback_only;
   if (prescreen) {
-    nown = (nraw - cx->rank + cx->world - 1) / cx->world;
+    nown = (nraw - scr_rank + scr_world - 1) / scr_world;
     kbits.alloc((size_t)nown * 32 + 32); kmeta.alloc(nown); krep.alloc((size_t)nown * 48 + 64); cand_list.alloc(nown + 32); cand_ms.alloc(nown + 32);
     old_list.alloc(nown + 32);
     if (kbits_gen != cx->upload_gen) {       // the bitmaps and repeat lists depend on the sequences only: kept across the runs of a resident sample
       d_novf.alloc(1); d_novf.zero(s);
-      launch_kmer_bits(in, cx->rank, cx->world, nown, kbits.p, kmeta.p, krep.p, d_novf.p, cx->num_sms, s);
+      launch_kmer_bits(in, scr_rank, scr_world, nown, kbits.p, kmeta.p, krep.p, d_novf.p, scr_sms, s);
       d2h(&n_ovf, d_novf.p, 4);            // read by the sync() at the end of alloc_state
       kbits_gen = cx->upload_gen;
     }
@@ -865,6 +884,34 @@ void Run::launch_align_jobs(int mode, AlignArgs &a, unsigned long long upper) {
   launch_align(mode, a, grid, 128, align_smem, s);
 }
 
+// raw_align's k-mer screen (nwalign_endsfree.cpp:44-56) of centre c against every raw of the shard, greedy skip included
+// (cluster.cpp:127-131): shrouded pairs are counted into CTR_ALIGN / CTR_SHROUD, the others are appended to st.gl_list / st.nw_list
+// (CTR_GL / CTR_NW).  The caller has zeroed the round's counters.  Used by the round and by the stage hook dada2b_test_screen.
+void Run::launch_screen(uint32_t c, uint32_t centre_reads, bool greedy, double kdist_cutoff, bool streaming) {
+  ClassifyArgs ca{};
+  ca.in = in; ca.P = P; ca.P.kdist_cutoff = kdist_cutoff; ca.mode = 0; ca.centre_idx = c; ca.centre_reads = centre_reads;
+  ca.greedy = greedy; ca.lock = st.lock; ca.nw_list = st.nw_list; ca.gl_list = st.gl_list; ca.ctr = st.ctr;
+  ca.kind_out = nullptr; ca.kord_words = kord_words; ca.shard_rank = scr_rank; ca.shard_world = scr_world;
+  int cgrid = std::min((nraw / scr_world + 8) / 8, scr_sms * 4);
+  if (streaming) {
+    // stream the 128-byte bitmap rows (TMA): every pair decided exactly (presence bound, then the exact min-sum through the raw's
+    // repeated-5-mer list); gapless / NW for the pairs that are not shrouded (k_kord); the warp-per-pair screen only sees raws
+    // whose list overflowed
+    ca.cand_list = old_list.p; ca.cand_count = st.ctr + CTR_OLD;
+    timed(T_PRE, [&]() {
+      launch_prescreen(in, kbits.p, kmeta.p, krep.p, nown, scr_rank, scr_world, c, centre_reads, greedy, st.lock, kdist_cutoff, cand_list.p,
+                       cand_ms.p, st.ctr + CTR_CAND, st.ctr, scr_sms, s);
+    });
+    prescreen_rows += nown;
+    timed(T_CLASSIFY, [&]() {
+      launch_kord(in, ca.P, c, cand_list.p, cand_ms.p, st.ctr + CTR_CAND, st.nw_list, st.gl_list, old_list.p, st.ctr + CTR_OLD, st.ctr, (unsigned long long)nown,
+                  scr_sms, s);
+      if (n_ovf) launch_classify(ca, std::min(cgrid, scr_sms), 256, classify_smem, s);      // only raws whose list overflowed can be forwarded
+    });
+  } else
+  timed(T_CLASSIFY, [&]() { launch_classify(ca, cgrid, 256, classify_smem, s); });
+}
+
 // One round on the device, no host round trip inside:
 //   [apply previous bud] -> b_compare_parallel (cluster.cpp:152-204) -> NP x b_shuffle2 -> b_p_update -> b_bud scan -> report
 void Run::launch_compare(uint32_t i, double kdist_cutoff) {
@@ -872,31 +919,10 @@ void Run::launch_compare(uint32_t i, double kdist_cutoff) {
   ensure_cs_cap(cs_count + 2ull * (unsigned long long)nraw + 1024);
   ensure_cluster_cap((size_t)nclust_h + 2);
   tail_sync_caps();
-  launch_round_begin(st, pending.apply, pending.r, pending.from, pending.newi, pending.reads, s);
+  launch_round_begin(st, pending.apply, pending.r, pending.from, pending.newi, pending.reads, s);      // zeroes the round's counters
   pending.apply = 0;
   count_round = true;
-  ClassifyArgs ca{};
-  ca.in = in; ca.P = P; ca.P.kdist_cutoff = kdist_cutoff; ca.mode = 0; ca.centre_idx = c; ca.centre_reads = cx->reads[c];
-  ca.greedy = o->greedy != 0; ca.lock = st.lock; ca.nw_list = st.nw_list; ca.gl_list = st.gl_list; ca.ctr = st.ctr;
-  ca.kind_out = nullptr; ca.kord_words = kord_words; ca.shard_rank = cx->rank; ca.shard_world = cx->world;
-  int cgrid = std::min((nraw / cx->world + 8) / 8, cx->num_sms * 4);
-  if (prescreen && kdist_cutoff < 1.0) {
-    // stream the 128-byte bitmap rows (TMA): every pair decided exactly (presence bound, then the exact min-sum through the raw's
-    // repeated-5-mer list); gapless / NW for the pairs that are not shrouded (k_kord); the warp-per-pair screen only sees raws
-    // whose list overflowed
-    ca.cand_list = old_list.p; ca.cand_count = st.ctr + CTR_OLD;      // the round's counters were zeroed by k_round_begin
-    timed(T_PRE, [&]() {
-      launch_prescreen(in, kbits.p, kmeta.p, krep.p, nown, cx->rank, cx->world, c, cx->reads[c], o->greedy != 0, st.lock, kdist_cutoff, cand_list.p,
-                       cand_ms.p, st.ctr + CTR_CAND, st.ctr, cx->num_sms, s);
-    });
-    prescreen_rows += nown;
-    timed(T_CLASSIFY, [&]() {
-      launch_kord(in, ca.P, c, cand_list.p, cand_ms.p, st.ctr + CTR_CAND, st.nw_list, st.gl_list, old_list.p, st.ctr + CTR_OLD, st.ctr, (unsigned long long)nown,
-                  cx->num_sms, s);
-      if (n_ovf) launch_classify(ca, std::min(cgrid, cx->num_sms), 256, classify_smem, s);      // only raws whose list overflowed can be forwarded
-    });
-  } else
-  timed(T_CLASSIFY, [&]() { launch_classify(ca, cgrid, 256, classify_smem, s); });
+  launch_screen(c, cx->reads[c], o->greedy != 0, kdist_cutoff, prescreen && kdist_cutoff < 1.0);
   bool fwd_done = false;
   bool fb_possible = false;   // only k_nwfwd hands pairs back (those that do not fit its register band)
   if (P.band >= 0) {       // register-resident NW kernels (dd_nwrow.cu / dd_nwlane.cu / dd_nwfwd.cu); unbanded pairs: k_align below
@@ -1653,7 +1679,7 @@ dada2b_out *do_run(dada2b_ctx *cx, const double *err_cm, int Q, const dada2b_opt
   if (!cx->run) cx->run = new Run();
   Run &R = *cx->run;
   R.reset_host();
-  R.cx = cx; R.o = o; R.s = cx->stream; R.in = cx->in; R.nraw = cx->in.nraw; R.ncol = Q;
+  R.bind(cx, o, Q);
   DBG("run: begin");
   cx->ev_next = 0;
   R.launches0 = launches_count();
@@ -1764,7 +1790,7 @@ static void do_test_pairs(dada2b_ctx *cx, int npairs, const uint32_t *centre, co
   CK(cudaSetDevice(cx->device));
   if (cx->bad_nt) throw Err{"Unexpected nucleotide."};
   Run R;
-  R.cx = cx; R.o = o; R.s = cx->stream; R.in = cx->in; R.nraw = cx->in.nraw; R.ncol = Q;
+  R.bind(cx, o, Q);
   R.setup_params();
   R.alloc_state();
   std::vector<double> e((size_t)16 * Q);
@@ -1821,7 +1847,7 @@ static void do_test_loop_nw(dada2b_ctx *cx, int which, int npairs, const uint32_
   CK(cudaSetDevice(cx->device));
   if (cx->bad_nt) throw Err{"Unexpected nucleotide."};
   Run R;
-  R.cx = cx; R.o = o; R.s = cx->stream; R.in = cx->in; R.nraw = cx->in.nraw; R.ncol = Q;
+  R.bind(cx, o, Q);
   R.setup_params();
   R.alloc_state();
   cudaStream_t s = R.s;
@@ -1866,7 +1892,55 @@ static void do_test_loop_nw(dada2b_ctx *cx, int which, int npairs, const uint32_
   }
 }
 
-static void do_test_calc_pA(int n, const int32_t *reads, const double *E, const int32_t *prior, double *out) {
+// The k-mer screen of one round (include/dada2b_test.h): Run::launch_screen, the round's own launch sequence, for shard (rank, world)
+// with the bitmaps of that shard built into this call's Run; the per-raw decision is read back from the gapless / NW lists.
+static void do_test_screen(dada2b_ctx *cx, uint32_t centre, const dada2b_opts *o, double kdist_cutoff, uint32_t centre_reads, const uint8_t *lock,
+                           int rank, int world, int max_sms, int path, int32_t *kind, int32_t *minsum, int64_t *counters) {
+  CK(cudaSetDevice(cx->device));
+  if (cx->bad_nt) throw Err{"Unexpected nucleotide."};
+  if (world < 1 || rank < 0 || rank >= world) throw Err{"dada2b_test_screen: bad rank/world"};
+  if (path != 0 && path != 1) throw Err{"dada2b_test_screen: path must be 0 (product selection) or 1 (k_classify)"};
+  if (max_sms < 0) throw Err{"dada2b_test_screen: max_sms must be >= 0"};
+  if (centre >= (uint32_t)cx->in.nraw) throw Err{"dada2b_test_screen: centre out of range"};
+  Run R;
+  R.bind(cx, o, 1);                                      // nothing is aligned: one quality column sizes the unused error table
+  R.scr_rank = rank; R.scr_world = world;
+  if (max_sms > 0) R.scr_sms = std::min(R.scr_sms, max_sms);
+  R.setup_params();
+  R.alloc_state();                                       // zeroes the counters and the locks, builds the shard's bitmaps
+  const size_t n = (size_t)R.nraw;
+  if (lock) R.h2d(R.lock.p, lock, n);
+  const bool streaming = path == 0 && R.prescreen && kdist_cutoff < 1.0;
+  R.launch_screen(centre, centre_reads, o->greedy != 0, kdist_cutoff, streaming);
+  R.read_ctr();
+  R.check_dev_error();
+  const unsigned long long ngl = R.h_ctr.p[CTR_GL], nnw = R.h_ctr.p[CTR_NW], ncand = streaming ? R.h_ctr.p[CTR_CAND] : 0;
+  if (ngl + nnw > n || ncand > (unsigned long long)R.nown) throw Err{"dada2b_test_screen: list count out of range"};
+  std::vector<uint32_t> gl(ngl), nw(nnw), cand(ncand);
+  std::vector<uint16_t> cms(ncand);
+  R.d2h(gl.data(), R.st.gl_list, ngl * 4); R.d2h(nw.data(), R.st.nw_list, nnw * 4);
+  R.d2h(cand.data(), R.cand_list.p, ncand * 4); R.d2h(cms.data(), R.cand_ms.p, ncand * 2);
+  R.sync();
+  for (size_t r = 0; r < n; r++) { kind[r] = (int)(r % world) == rank ? 0 : -1; minsum[r] = -1; }
+  auto owned = [&](uint32_t r) {
+    if (r >= n || kind[r] < 0) throw Err{"dada2b_test_screen: a raw of another rank was screened"};
+  };
+  for (int k : {KIND_GAPLESS, KIND_NW})
+    for (uint32_t r : k == KIND_GAPLESS ? gl : nw) {
+      owned(r);
+      if (kind[r] != 0) throw Err{"dada2b_test_screen: a raw appears twice in the gapless / NW lists"};
+      kind[r] = k;
+    }
+  for (size_t k = 0; k < ncand; k++) {
+    owned(cand[k]);
+    if (minsum[cand[k]] != -1) throw Err{"dada2b_test_screen: a raw appears twice in the candidate list"};
+    minsum[cand[k]] = cms[k];
+  }
+  counters[0] = (int64_t)R.h_ctr.p[CTR_ALIGN]; counters[1] = (int64_t)R.h_ctr.p[CTR_SHROUD];
+  counters[2] = (int64_t)ngl; counters[3] = (int64_t)nnw;
+}
+
+static void do_test_calc_pA(int n,const int32_t *reads, const double *E, const int32_t *prior, double *out) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) throw Err{"dada2b: no CUDA device available (this library has no CPU path)."};
   DBuf<int> r, p; DBuf<double> e, o;
@@ -1893,6 +1967,13 @@ int dada2b_test_pairs(dada2b_ctx *ctx, int32_t npairs, const uint32_t *centre, c
 int dada2b_test_loop_nw(dada2b_ctx *ctx, int32_t which, int32_t npairs, const uint32_t *centre, const uint32_t *raw, const double *err,
                         int32_t Q, const dada2b_opts *opts, double *lambda, int32_t *nsubs, int32_t *handled, char errbuf[DADA2B_ERRLEN]) {
   try { do_test_loop_nw(ctx, which, npairs, centre, raw, err, Q, opts, lambda, nsubs, handled); return 0; }
+  catch (Err &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.msg.c_str()); return 1; }
+  catch (std::exception &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.what()); return 2; }
+}
+int dada2b_test_screen(dada2b_ctx *ctx, uint32_t centre, const dada2b_opts *opts, double kdist_cutoff, uint32_t centre_reads,
+                       const uint8_t *lock, int32_t rank, int32_t world, int32_t max_sms, int32_t path, int32_t *kind, int32_t *minsum,
+                       int64_t *counters, char errbuf[DADA2B_ERRLEN]) {
+  try { do_test_screen(ctx, centre, opts, kdist_cutoff, centre_reads, lock, rank, world, max_sms, path, kind, minsum, counters); return 0; }
   catch (Err &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.msg.c_str()); return 1; }
   catch (std::exception &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.what()); return 2; }
 }

@@ -34,6 +34,19 @@ int dada2b_test_calc_pA(int32_t n, const int32_t *reads, const double *E, const 
 int dada2b_test_loop_nw(dada2b_ctx *ctx, int32_t which, int32_t npairs, const uint32_t *centre, const uint32_t *raw, const double *err,
                         int32_t Q, const dada2b_opts *opts, double *lambda, int32_t *nsubs, int32_t *handled, char errbuf[DADA2B_ERRLEN]);
 
+/* Stage hook for the k-mer screen of one round (raw_align's shroud / gapless / NW decision, nwalign_endsfree.cpp:44-56, with the
+ * greedy skip of cluster.cpp:127-131): centre `centre` against every raw r with r % world == rank, through the round's own launch
+ * sequence.  opts->greedy, centre_reads and lock[nraw] (NULL: no raw locked) drive the skip; kdist_cutoff is passed separately, as
+ * in the round.  max_sms caps the SM count the launches size their grids from (0: the context's).  path 0 is the product's selection
+ * (k_prescreen -> k_kord, k_classify for raws whose repeat list overflowed; k_classify alone when kdist_cutoff >= 1), path 1
+ * k_classify alone.  Per raw, nraw entries each:
+ *   kind[r]   -1 raw of another rank, 0 neither gapless nor NW (shrouded or skipped), 1 gapless, 2 NW
+ *   minsum[r] the min-sum k_prescreen handed on (0xFFFF: repeat list overflowed), -1 when the raw was no candidate
+ * counters: CTR_ALIGN, CTR_SHROUD, CTR_GL, CTR_NW of the round.  Fails when a raw appears twice or a raw of another rank appears. */
+int dada2b_test_screen(dada2b_ctx *ctx, uint32_t centre, const dada2b_opts *opts, double kdist_cutoff, uint32_t centre_reads,
+                       const uint8_t *lock, int32_t rank, int32_t world, int32_t max_sms, int32_t path, int32_t *kind, int32_t *minsum,
+                       int64_t *counters, char errbuf[DADA2B_ERRLEN]);
+
 #ifdef __cplusplus
 }
 #endif

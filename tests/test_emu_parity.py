@@ -79,6 +79,27 @@ def test_emu_e2e(emu, name):
     _gpu_tests().test_e2e_matches_reference_golden(name)
 
 
+@pytest.mark.parametrize("name", ["syn2000_default", "syn700_ragged", "syn800_nogreedy"])
+def test_emu_e2e_one_sm(emu, monkeypatch, name):
+    """CUEMU_SMS=1: one emulated SM, so every CTA of the grid-stride kernels takes several tiles / jobs (the streaming screen's ring
+    stages are reused, pending raws are handed across tiles); goldens and screen counts stay the reference's."""
+    monkeypatch.setenv("CUEMU_SMS", "1")
+    monkeypatch.setenv("DADA2B_SMS", "1")
+    _gpu_tests().test_e2e_golden_at_capped_sm_count(monkeypatch, name, "1")
+
+
+@pytest.mark.parametrize("sms", ["1", "2"])
+def test_emu_screen_stage(emu, monkeypatch, sms):
+    """tests/screen_cases.py through the stage hook dada2b_test_screen on both paths, against tests/screen_ref.py (the GPU suite runs the
+    same cases in test_gpu_zz_screen.py, plus a 250 k-raw full-grid case that is too slow here)."""
+    import dada2_b200.api as api
+    from tests import screen_cases as SC
+    monkeypatch.setenv("CUEMU_SMS", sms)
+    for case in SC.small_cases():
+        SC.run_case(api.Resident, case, int(sms))
+    assert emu.cuemu_launches(b"k_prescreen") > 0 and emu.cuemu_launches(b"k_kord") > 0 and emu.cuemu_launches(b"k_classify") > 0
+
+
 @pytest.mark.parametrize("name", ["syn800_default", "syn800_band8", "syn800_kdist"] if not os.environ.get("DADA2B_EMU_FULL") else list(cases.E2E_CASES))
 def test_emu_e2e_fallback_kernels(emu, monkeypatch, name):
     """DADA2B_FALLBACK=1: no thread-per-pair / lane kernels, no streaming screen -- the general kernels alone (the path of

@@ -43,3 +43,27 @@ def test_1e5_uniques_invariants_determinism_and_paths_agree():
     cases.assert_same(got, load_golden("fullsize_1e5"), rtol=1e-10, label="1e5 uniques vs the reference's C++")
     st = a["stats"]
     assert st["gpu_launches"] > 1000 and st["n_nw"] > 1_000_000 and st["n_final_nw"] == 100000
+    cases.assert_same_screen_counts(a, oracle_counts(), label="1e5 uniques")
+
+
+def oracle_counts():
+    """The k-mer screen's totals on this workload from the CPU oracle (tools/make_golden_fuzz.py)."""
+    import json
+    import os
+    return json.load(open(os.path.join(cases.GOLDEN, "e2e_fullsize_1e5_counts.json")))
+
+
+def test_1e5_uniques_at_three_sms(monkeypatch):
+    """DADA2B_SMS=3: the streaming screen runs 9 CTAs over 782 tiles (about 87 per CTA, the 4-stage ring wraps about 21 times) and
+    every grid-stride kernel of the round takes many jobs per thread; output and screen counts stay the reference's."""
+    import dada2_b200
+    from tests.test_oracle import load_golden
+    monkeypatch.setenv("DADA2B_SMS", "3")
+    seqs, ab, q, err, truth = workload()
+    res = dada2_b200.Resident(seqs, ab, None, q)
+    a = res.run(err)
+    res.close()
+    idx = sample_raws(len(seqs))
+    got = dict(a, map=np.asarray(a["map"])[idx], pval=np.asarray(a["pval"])[idx])
+    cases.assert_same(got, load_golden("fullsize_1e5"), rtol=1e-10, label="1e5 uniques at 3 SMs")
+    cases.assert_same_screen_counts(a, oracle_counts(), label="1e5 uniques at 3 SMs")

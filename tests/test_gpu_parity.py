@@ -147,6 +147,7 @@ def test_config1_bit_identical():
     want = load_golden("config1")
     cases.assert_same(got, want, rtol=1e-10, label="config1")
     assert len(got["clustering"]["sequence"]) == 10
+    assert (got["stats"]["n_align"], got["stats"]["n_shroud"]) == (8655, 3032)          # the oracle's counts (tests/test_oracle.py)
 
 
 @pytest.mark.parametrize("name", sorted(cases.E2E_CASES))
@@ -154,12 +155,40 @@ def test_e2e_matches_reference_golden(name):
     api = _api()
     seqs, ab, pri, err, q, opts = cases.build_case(name)
     got = api.dada_uniques(seqs, ab, pri, err, q, **opts)
+    _check_e2e(name, got)
+
+
+def _check_e2e(name, got):
+    seqs, ab, pri, err, q, opts = cases.build_case(name)
     want = load_golden(name)
     pb = None
     if pri is not None:
         pb = np.zeros(len(want["clustering"]["sequence"]), dtype=bool)
         pb[1:] = want["clustering"]["birth_pval"][1:] >= opts.get("omegaA", 1e-40)
     cases.assert_same(got, want, rtol=1e-10, prior_born=pb, label=name)
+    cases.assert_same_screen_counts(got, cases.oracle_screen_counts(name), label=name)
+
+
+@pytest.mark.parametrize("sms", ["1", "2"])
+@pytest.mark.parametrize("name", sorted(cases.E2E_CASES) + ["config1"])
+def test_e2e_golden_at_capped_sm_count(monkeypatch, name, sms):
+    """DADA2B_SMS (test hook, read at upload) caps the SM count every grid of dada() is sized from: golden-sized inputs then give each
+    CTA many tiles / jobs (the streaming screen's ring wraps, grid-stride loops run several times), as the 1e6 workload does."""
+    api = _api()
+    monkeypatch.setenv("DADA2B_SMS", sms)
+    if name == "config1":
+        seqs, ab, q = cases.load_config1()
+        res = api.Resident(seqs, ab, None, q)
+        got = res.run(cases.tperr1())
+        res.close()
+        cases.assert_same(got, load_golden("config1"), rtol=1e-10, label="config1 at %s SMs" % sms)
+        assert (got["stats"]["n_align"], got["stats"]["n_shroud"]) == (8655, 3032)
+        return
+    seqs, ab, pri, err, q, opts = cases.build_case(name)
+    res = api.Resident(seqs, ab, pri, q)
+    got = res.run(err, **opts)
+    res.close()
+    _check_e2e(name, got)
 
 
 @pytest.mark.parametrize("blk", [1, 100])

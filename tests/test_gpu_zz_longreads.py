@@ -26,6 +26,7 @@ SCRIPT = textwrap.dedent('''
         got = dada2_b200.dada_uniques(seqs, ab, None, err, q, **opts)
         want = port.dada_uniques(seqs, ab, None, err, q, **o)
         cases.assert_same(got, want, rtol=1e-10, label=str(opts))
+        cases.assert_same_screen_counts(got, want, label=str(opts))
     print("LONGREADS OK")
 ''') % ROOT
 

@@ -16,4 +16,5 @@ def test_large_tie_sets_follow_scan_order(opts):
     got = dada2_b200.dada_uniques(seqs, ab, None, err, q, **opts)
     want = port.dada_uniques(seqs, ab, None, err, q, **dict(opts, homo_gap=-8))
     cases.assert_same(got, want, rtol=1e-10, label="ties " + str(opts))
+    cases.assert_same_screen_counts(got, want, label="ties " + str(opts))
     assert len(got["clustering"]["abundance"]) == (30 if "max_clust" in opts else 151)

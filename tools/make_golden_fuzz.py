@@ -5,7 +5,10 @@
     bimera_fuzz.npz       ref.table_bimera() / ref.bimera_pair() on tests/test_bimera_oracle.py's fuzz cases
     e2e_fullsize_1e5.npz  ref.dada_uniques() on tests/test_gpu_fullsize.py's 1e5 uniques; map and pval at its seeded
                           sample of raws (sample_raws), so that the file stays small
-Run:  python tools/make_golden_fuzz.py"""
+    e2e_fullsize_1e5_counts.json  the k-mer screen's totals on the same 1e5 uniques (n_align, n_shroud) from the CPU
+                          oracle (oracle/port.cpp), which counts them with the reference's serial semantics
+Run:  python tools/make_golden_fuzz.py  (--counts-only: the counts fixture alone)"""
+import json
 import os
 import sys
 
@@ -18,7 +21,21 @@ from tests import cases, test_bimera_oracle as TB, test_oracle_fuzz as TF, test_
 from tools.make_golden import save_res               # noqa: E402
 
 
+def fullsize_counts():
+    from oracle import port
+    seqs, ab, q, err, _ = TG.workload()
+    st = port.dada_uniques(seqs, ab, None, err, q, homo_gap=-8)["stats"]
+    path = os.path.join(cases.GOLDEN, "e2e_fullsize_1e5_counts.json")
+    with open(path, "w") as f:
+        json.dump({"n_align": int(st["n_align"]), "n_shroud": int(st["n_shroud"])}, f)
+        f.write("\n")
+    print(path, open(path).read().strip())
+
+
 def main():
+    fullsize_counts()
+    if "--counts-only" in sys.argv:
+        return
     G = cases.GOLDEN
     err = cases.tperr1()
     cols = {k: [] for k in ("shrouded", "lam", "nsubs", "al0", "al1") + TF.PAIR_ARRAYS}
