@@ -47,8 +47,8 @@ enum Ctr : int {
 constexpr int TIE_MAX = 64;      // tie candidates reported per round without a second copy
 constexpr int MAX_PASS = 10;     // MAX_SHUFFLE, /root/reference/src/dada.h:30
 
-// Written by the device into mapped pinned host memory once per round; read by the host after a
-// single stream synchronisation (no per-step D2H copies).
+// Written by the device (k_tail_final) once per round, at the head of the buffer that also holds the round's move list; the
+// host copies it back together with the head of the move list after a single stream synchronisation.
 struct RoundReport {
   unsigned long long ctr[CTR_N];
   uint32_t pinfo[MAX_PASS + 2];   // pinfo[p+1] = moves recorded up to and including shuffle pass p
@@ -56,8 +56,8 @@ struct RoundReport {
   uint32_t pad;
   uint32_t tie_r[TIE_MAX], tie_ham[TIE_MAX], tiep_r[TIE_MAX], tiep_ham[TIE_MAX];
   double tie_lam[TIE_MAX], tiep_lam[TIE_MAX];
-  // fused tail only: cluster of every tie candidate and that cluster's reads after the last pass, so that the host can open the
-  // next round before it has replayed this round's moves on its member arrays (dd_driver.cu: replay worker)
+  // cluster of every tie candidate and that cluster's reads after the last pass, so that the host can open the next round
+  // before it has replayed this round's moves on its member arrays (dd_driver.cu: replay worker)
   uint32_t tie_cl[TIE_MAX], tie_clreads[TIE_MAX], tiep_cl[TIE_MAX], tiep_clreads[TIE_MAX];
 };
 
@@ -73,11 +73,8 @@ struct DevState {
   double *cs_lambda;
   unsigned long long cs_cap;
   // per cluster
-  uint32_t *cl_reads, *cl_reads_next, *cl_center;
+  uint32_t *cl_reads, *cl_center;
   uint8_t *cl_update_e, *cl_check_locks;
-  // shuffle scratch (per raw)
-  unsigned long long *emax_bits;
-  uint32_t *best_entry;
   // job lists
   uint32_t *nw_list, *gl_list;
   // device counters / flags (see enum Ctr)
@@ -86,11 +83,11 @@ struct DevState {
   double *err;
   // sharded runs (one process per GPU): raw r is owned by rank r % shard_world
   int shard_rank, shard_world;
-  // per-round control block (device) + host-mapped report / move list
+  // per-round control block, report and move list (device memory; report and moves are views of one buffer)
   uint32_t *pinfo;                  // [MAX_PASS + 2]
-  uint32_t *moves;                  // mapped pinned host memory: (raw, to) pairs
+  uint32_t *moves;                  // [move_cap] (raw, to) pairs
   unsigned move_cap;
-  RoundReport *report;              // mapped pinned host memory
+  RoundReport *report;
   // final-pass accumulators
   int *trans;                       // [16][ncol] row-major
   unsigned long long *cq_sum, *cq_cnt;  // [nclust][maxlen]

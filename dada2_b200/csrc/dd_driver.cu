@@ -484,30 +484,25 @@ struct Run {
   // device state buffers
   DBuf<uint8_t> lock, is_center, slot0, correct, cl_update_e, cl_check_locks, b_nt0, b_nt1, b_q1, b_ops, kind_out;
   DBuf<double> E_minmax, p, comp_lambda, cs_lambda, err, b_lambda, trip_v, pa_E, pa_out;
-  DBuf<uint32_t> comp_ham, cluster_of, cs_index, cs_i, cs_ham, cl_reads, cl_center, best_entry, nw_list, gl_list,
+  DBuf<uint32_t> comp_ham, cluster_of, cs_index, cs_i, cs_ham, cl_reads, cl_center, nw_list, gl_list,
       nsubs_final, ptr_scratch, pair_centre, pair_raw, b_nsubs, b_nops, trip_ij;
   DBuf<uint16_t> b_pos;
-  DBuf<unsigned long long> emax_bits, ctr, cq_sum, cq_cnt;
+  DBuf<unsigned long long> ctr, cq_sum, cq_cnt;
   DBuf<int> trans, center_cluster, pa_reads, pa_prior;
   PBuf<unsigned long long> h_ctr;
-  DBuf<uint32_t> cl_reads_next, pinfo;
-  DBuf<RoundReport> d_report;
-  DBuf<uint32_t> d_moves;
-  // Owner mode: report and move list share ONE device buffer [RoundReport | moves], so that the round's all-gather carries the report
-  // together with the first `eager_sh` moves of every rank: the move lists need a collective of their own only in the few rounds that
-  // move more (one NCCL call + one host synchronisation less per round).
+  DBuf<uint32_t> pinfo;
+  // Report and move list share ONE device buffer [RoundReport | moves], so that the round's copy back (sharded: its all-gather)
+  // carries the report together with the first `eager` moves of every rank: the move lists need a copy (collective) of their own
+  // only in the few rounds that move more (one call + one host synchronisation less per round).
   DBuf<uint8_t> d_repmv, d_gather_all;
   PBuf<uint8_t> h_gather_all;
   static constexpr size_t RR_PAD = (sizeof(RoundReport) + 15) & ~(size_t)15;
-  unsigned eager_sh = 1024;
-  RoundReport *rep_dev = nullptr;        // where the device writes the report / the moves (views of d_repmv in owner mode)
-  uint32_t *mv_dev = nullptr;
-  std::vector<const RoundReport *> rep_all;   // owner mode: every rank's report of the round (pinned host copy)
+  unsigned eager = 0;
+  std::vector<const RoundReport *> rep_all;   // every rank's report of the round (pinned host copy)
   PBuf<RoundReport> h_report_buf;
   PBuf<uint32_t> h_moves_buf;
-  RoundReport *h_report = nullptr;       // pinned host copy, refreshed once per round
+  RoundReport *h_report = nullptr;       // the ranks' reports merged, refreshed once per round
   uint32_t *h_moves = nullptr;
-  static constexpr unsigned MOVES_EAGER = 8192;   // moves copied back with the report; more => one extra copy
   int NP = 3;                            // shuffle passes launched speculatively per round
   unsigned move_cap = 0;
   DBuf<uint32_t> fb_list, surv_list, uneq_list;
@@ -540,16 +535,13 @@ struct Run {
   int scr_rank = 0, scr_world = 1, scr_sms = 1;
   bool fallback_only = false;         // DADA2B_FALLBACK (test switch): general kernels only
   bool two_phase = false;              // bound pass first, exact lambda for the survivors only (plain gap costs)
-  // fused round tail (experimental, DADA2B_FUSED_TAIL=1; dd_round2.cu)
-  bool fused_tail = false;               // dd_round2.cu: link + NP passes + final (default); dd_round.cu's split tail otherwise
-  // owner mode (sharded runs, on top of the fused tail): every rank keeps the stored comparisons and
-  // runs shuffle / p-update / bud scan for its own raws only; per pass one all-reduce of the cluster read deltas, per round one
-  // all-gather of the ranks' reports (bud candidates, move counts) and, when raws moved, one of the move lists.
-  bool owner = false;
+  // round tail (dd_round2.cu): every rank keeps the stored comparisons and runs shuffle / p-update / bud scan for its own raws
+  // only (one rank: every raw); sharded runs add per pass one all-reduce of the cluster read deltas, per round one all-gather of
+  // the ranks' reports (bud candidates, move counts) and, when raws moved, one of the move lists.
   int tail_last = -1;                    // last shuffle pass launched in the current round
+  int tail_smem_clusters = 0;            // rounds with at most this many clusters stage the tail's per-cluster state in shared memory
   DBuf<uint32_t> d_moves_all;
   PBuf<uint32_t> h_moves_all;
-  void sync_report_owner();
   TailState ts{};
   DBuf<uint32_t> t_head, t_prev, t_nmove, t_bt, t_btp;
   DBuf<int> t_delta;
@@ -568,7 +560,7 @@ struct Run {
   std::vector<Birth> birth;
   int nclust_h = 0;
   // b_shuffle2's container updates and b_bud's pop / new cluster are pure host bookkeeping (O(moves), but ~30 ms of a 1e6-unique
-  // run): with the fused tail the device reports everything the next bud decision needs unless it is an exact tie, so the updates
+  // run): the device reports everything the next bud decision needs unless it is an exact tie, so the updates
   // are queued to a worker and applied while the GPU runs the next round.
   struct ReplayEvent { int kind; std::vector<uint32_t> mv; std::vector<uint32_t> pass_end; uint32_t r, from, ni; };
   bool async_replay = false;
@@ -656,8 +648,6 @@ struct Run {
   void launch_compare(uint32_t i, double kdist_cutoff);
   void launch_round_tail(int first_pass, int npass);
   void launch_round_tail_inner(int first_pass, int npass);
-  void launch_shuffle_only(int pass);
-  void launch_round_tail_noshuffle();
   void sync_report();
   int replay_moves(int first_pass, int last_pass);
   int decide_bud(uint32_t *r_out, uint32_t *from_out);
@@ -712,9 +702,8 @@ void Run::setup_params() {
   if (classify_smem > 100 * 1024) throw Err{"dada2b: sequences too long for the k-mer screen kernel."};
 }
 
-// Keeps the fused tail's per-entry / per-cluster arrays as large as the comparison store and the cluster arrays.
+// Keeps the round tail's per-entry / per-cluster arrays as large as the comparison store and the cluster arrays.
 void Run::tail_sync_caps() {
-  if (!fused_tail) return;
   if (t_prev.n < st.cs_cap) {
     DBuf<uint32_t> np;
     np.alloc(st.cs_cap);
@@ -725,27 +714,25 @@ void Run::tail_sync_caps() {
   const size_t stride = 2 * cl_cap + 4;
   if (t_delta.n < (size_t)MAX_PASS * stride) { t_delta.alloc((size_t)MAX_PASS * stride); t_delta.zero(s); }   // cleared every round by k_tail_link
   ts.cs_prev = t_prev.p; ts.rows = t_delta.p; ts.cl_cap = (uint32_t)cl_cap; ts.row_stride = (uint32_t)stride;
-  ts.rank = owner ? cx->rank : 0; ts.world = owner ? cx->world : 1;
 }
 
 void Run::ensure_cluster_cap(size_t n) {
   if (n <= cl_cap) return;
   size_t nc = std::max<size_t>(1024, cl_cap * 2);
   while (nc < n) nc *= 2;
-  DBuf<uint32_t> r2, rn2, c2; DBuf<uint8_t> u2, k2;
-  r2.alloc(nc); rn2.alloc(nc); c2.alloc(nc); u2.alloc(nc); k2.alloc(nc);
-  r2.zero(s); rn2.zero(s); c2.zero(s); u2.zero(s); k2.zero(s);
+  DBuf<uint32_t> r2, c2; DBuf<uint8_t> u2, k2;
+  r2.alloc(nc); c2.alloc(nc); u2.alloc(nc); k2.alloc(nc);
+  r2.zero(s); c2.zero(s); u2.zero(s); k2.zero(s);
   if (cl_cap) {
     CK(cudaMemcpyAsync(r2.p, cl_reads.p, cl_cap * 4, cudaMemcpyDeviceToDevice, s));
-    CK(cudaMemcpyAsync(rn2.p, cl_reads_next.p, cl_cap * 4, cudaMemcpyDeviceToDevice, s));
     CK(cudaMemcpyAsync(c2.p, cl_center.p, cl_cap * 4, cudaMemcpyDeviceToDevice, s));
     CK(cudaMemcpyAsync(u2.p, cl_update_e.p, cl_cap, cudaMemcpyDeviceToDevice, s));
     CK(cudaMemcpyAsync(k2.p, cl_check_locks.p, cl_cap, cudaMemcpyDeviceToDevice, s));
   }
   sync();
-  cl_reads.swap(r2); cl_reads_next.swap(rn2); cl_center.swap(c2); cl_update_e.swap(u2); cl_check_locks.swap(k2);
+  cl_reads.swap(r2); cl_center.swap(c2); cl_update_e.swap(u2); cl_check_locks.swap(k2);
   cl_cap = nc;
-  st.cl_reads = cl_reads.p; st.cl_reads_next = cl_reads_next.p; st.cl_center = cl_center.p;
+  st.cl_reads = cl_reads.p; st.cl_center = cl_center.p;
   st.cl_update_e = cl_update_e.p; st.cl_check_locks = cl_check_locks.p;
 }
 
@@ -775,7 +762,7 @@ void Run::alloc_state() {
   arena_off = 0; pend.clear();
   lock.alloc(n); is_center.alloc(n); slot0.alloc(n); correct.alloc(n);
   E_minmax.alloc(n); p.alloc(n); comp_lambda.alloc(n); comp_ham.alloc(n); cluster_of.alloc(n);
-  emax_bits.alloc(n); best_entry.alloc(n); nw_list.alloc(n); gl_list.alloc(n); nsubs_final.alloc(n);
+  nw_list.alloc(n); gl_list.alloc(n); nsubs_final.alloc(n);
   TDBG("alloc: device arrays");
   ctr.alloc(CTR_N); h_ctr.alloc(CTR_N);
   DBG("alloc: ctr done");
@@ -807,26 +794,23 @@ void Run::alloc_state() {
     }
   }
   if (const char *e = getenv("DADA2B_NP")) NP = std::max(1, std::min(MAX_PASS, atoi(e)));      // tuning / test override
-  fused_tail = getenv("DADA2B_SPLIT_TAIL") == nullptr;   // test switch: the one-kernel-per-step tail of dd_round.cu (capacity fallback beyond 32 k clusters)
-  owner = cx->world > 1;           // sharded runs: every rank keeps / shuffles / scans its own raws only (needs the fused tail)
-  if (owner && !fused_tail) throw Err{"dada2b: sharded runs need the fused round tail (unset DADA2B_SPLIT_TAIL)"};
-  if (fused_tail) {
+  tail_smem_clusters = tail_smem_clusters_max();
+  if (const char *e = getenv("DADA2B_TAIL_SMEM_CLUSTERS"))     // test hook: 0 = every round's tail in global memory, as past ~32 k clusters
+    tail_smem_clusters = std::min(tail_smem_clusters, std::max(0, atoi(e)));
+  {
     const size_t g = (size_t)tail_grid(nraw);
     t_head.alloc(n); t_nmove.alloc(MAX_PASS); t_done.alloc(1); t_blk.alloc(g); t_bt.alloc(g * TIE_MAX); t_btp.alloc(g * TIE_MAX);
     t_nmove.zero(s); t_done.zero(s);
     ts.head = t_head.p; ts.nmove_pass = t_nmove.p; ts.done = t_done.p; ts.blk = t_blk.p; ts.blk_ties = t_bt.p; ts.blk_ties_pr = t_btp.p;
+    ts.rank = cx->rank; ts.world = cx->world;
   }
   pinfo.alloc(MAX_PASS + 2); pinfo.zero(s);
-  if (owner) {
-    d_repmv.alloc(RR_PAD + (size_t)move_cap * 8);
-    rep_dev = (RoundReport *)d_repmv.p; mv_dev = (uint32_t *)(d_repmv.p + RR_PAD);
-    eager_sh = 1024;
-    if (const char *e = getenv("DADA2B_MOVES_EAGER")) eager_sh = (unsigned)std::max(0, atoi(e));      // test hook: 0 = every move list through its own all-gather
-    eager_sh = std::min(eager_sh, move_cap);
-  } else {
-    d_report.alloc(1); d_moves.alloc((size_t)move_cap * 2);
-    rep_dev = d_report.p; mv_dev = d_moves.p;
-  }
+  d_repmv.alloc(RR_PAD + (size_t)move_cap * 8);
+  // Moves carried with the report.  One GPU: enough for nearly every round without a second copy.  Sharded: 1024 per rank (an
+  // untimed choice: the all-gather moves world times as much).
+  eager = cx->world > 1 ? 1024 : 8192;
+  if (const char *e = getenv("DADA2B_MOVES_EAGER")) eager = (unsigned)std::max(0, atoi(e));      // test hook: 0 = every move list through its own copy
+  eager = std::min(eager, move_cap);
   h_report_buf.alloc(1); h_moves_buf.alloc((size_t)move_cap * 2);
   h_report = h_report_buf.p; h_moves = h_moves_buf.p;
   memset(h_report, 0, sizeof(RoundReport));
@@ -839,22 +823,20 @@ void Run::alloc_state() {
   TDBG("alloc: synced");
   st.lock = lock.p; st.is_center = is_center.p; st.slot0 = slot0.p; st.correct = correct.p;
   st.E_minmax = E_minmax.p; st.p = p.p; st.comp_lambda = comp_lambda.p; st.comp_ham = comp_ham.p; st.cluster_of = cluster_of.p;
-  st.emax_bits = emax_bits.p; st.best_entry = best_entry.p; st.nw_list = nw_list.p; st.gl_list = gl_list.p;
+  st.nw_list = nw_list.p; st.gl_list = gl_list.p;
   st.ctr = ctr.p; st.err = err.p; st.nsubs_final = nsubs_final.p;
   st.pinfo = pinfo.p; st.move_cap = move_cap;
   st.shard_rank = cx->rank; st.shard_world = cx->world;
-  st.report = rep_dev; st.moves = mv_dev;
-  emax_bits.zero(s);                                               // shuffle scratch starts clean
-  CK(cudaMemsetAsync(best_entry.p, 0xFF, n * 4, s));
+  st.report = (RoundReport *)d_repmv.p; st.moves = (uint32_t *)(d_repmv.p + RR_PAD);
   { unsigned long long nn = n; h2d(ctr.p + CTR_CS_COUNT, &nn, 8); }  // cluster 0 owns entries [0, nraw)
   sync();
   st.cs_cap = 0;
   ensure_cs_cap(2ull * n + 1024);
   TDBG("alloc: cs cap");
   ensure_cluster_cap(1024);
-  st.cl_reads = cl_reads.p; st.cl_reads_next = cl_reads_next.p; st.cl_center = cl_center.p;
+  st.cl_reads = cl_reads.p; st.cl_center = cl_center.p;
   st.cl_update_e = cl_update_e.p; st.cl_check_locks = cl_check_locks.p;
-  cl_reads.zero(s); cl_reads_next.zero(s); cl_center.zero(s); cl_update_e.zero(s); cl_check_locks.zero(s);
+  cl_reads.zero(s); cl_center.zero(s); cl_update_e.zero(s); cl_check_locks.zero(s);
   sync();
   TDBG("alloc: cluster cap");
   if (!ptr_in_smem) {
@@ -987,7 +969,7 @@ void Run::launch_compare(uint32_t i, double kdist_cutoff) {
     a.centre_idx = c; a.centre_reads = cx->reads[c]; a.cluster_i = i; a.total_reads = cx->total_reads;
     timed(kind == KIND_NW ? T_NW : T_GL, [&]() { launch_align_jobs(MODE_LOOP, a, (unsigned long long)nraw); });
   }
-  if (fused_tail) launch_tail_link(st, ts, cs_count, i, nraw, nclust_h, s);
+  launch_tail_link(st, ts, cs_count, i, nraw, nclust_h, s);
 }
 
 // shuffle passes [first_pass, first_pass + npass) then p-update, bud scan and the report
@@ -996,53 +978,33 @@ void Run::launch_round_tail(int first_pass, int npass) {
 }
 void Run::launch_round_tail_inner(int first_pass, int npass) {
   const int nclust = nclust_h;
-  const unsigned long long upper = cs_count + (unsigned long long)nraw;
-  if (fused_tail && !tail_fits(nclust)) {       // per-cluster reads no longer fit shared memory: the split tail takes over for the rest of the run
-    if (owner) throw Err{"dada2b: too many clusters for a sharded run (the fused round tail holds per-cluster state in shared memory)"};
-    fused_tail = false;
-    drain_replay(); async_replay = false;       // the split tail does not report the candidates' clusters
+  const bool smem = nclust <= tail_smem_clusters;
+  for (int p = first_pass; p < first_pass + npass; p++) {
+    launch_tail_pass(st, in, ts, p, nclust, smem, s);
+    if (cx->world > 1) NC(g_nccl.AllReduce(ts.rows + (size_t)p * ts.row_stride, ts.rows + (size_t)p * ts.row_stride, ts.row_stride, ncclInt32, ncclSum, cx->comm, s));
   }
-  if (fused_tail) {
-    for (int p = first_pass; p < first_pass + npass; p++) {
-      launch_tail_pass(st, in, ts, p, nclust, s);
-      if (owner) NC(g_nccl.AllReduce(ts.rows + (size_t)p * ts.row_stride, ts.rows + (size_t)p * ts.row_stride, ts.row_stride, ncclInt32, ncclSum, cx->comm, s));
-    }
-    tail_last = first_pass + npass - 1;
-    BudParams bp{o->min_fold, o->min_hamming, o->min_abund};
-    bp.skip_log = log(o->omegaA / (double)(unsigned)nraw) + 1.0;                       // decide_bud: pA = p * nraw < omegaA
-    bp.skip_log_prior = log(std::max(o->omegaA / (double)(unsigned)nraw, o->omegaP)) + 1.0;   // ... or p < omegaP
-    if (!(bp.skip_log == bp.skip_log)) bp.skip_log = 1e300;                              // non-positive thresholds: no shortcut
-    if (!(bp.skip_log_prior == bp.skip_log_prior)) bp.skip_log_prior = 1e300;
-    launch_tail_final(st, in, ts, bp, o->greedy != 0, o->detect_singletons != 0, tail_last, nclust, tail_last == MAX_PASS - 1 ? 2 : 0, s);
-    return;
-  }
-  for (int p = first_pass; p < first_pass + npass; p++) launch_shuffle_pass(st, in, upper, nclust, p, s);
-  const int last = first_pass + npass - 1;          // -1 => no shuffling this round (initial cluster)
-  launch_p_update(st, in, o->greedy != 0, o->detect_singletons != 0, last, s);
+  tail_last = first_pass + npass - 1;          // -1 => no shuffling this round (initial cluster)
   BudParams bp{o->min_fold, o->min_hamming, o->min_abund};
-  launch_bud_scan(st, in, bp, nclust, last, s);
-  launch_report(st, last, s);
+  bp.skip_log = log(o->omegaA / (double)(unsigned)nraw) + 1.0;                       // decide_bud: pA = p * nraw < omegaA
+  bp.skip_log_prior = log(std::max(o->omegaA / (double)(unsigned)nraw, o->omegaP)) + 1.0;   // ... or p < omegaP
+  if (!(bp.skip_log == bp.skip_log)) bp.skip_log = 1e300;                              // non-positive thresholds: no shortcut
+  if (!(bp.skip_log_prior == bp.skip_log_prior)) bp.skip_log_prior = 1e300;
+  launch_tail_final(st, in, ts, bp, o->greedy != 0, o->detect_singletons != 0, tail_last, nclust, tail_last == MAX_PASS - 1 ? 2 : 0, smem, s);
 }
 
-void Run::launch_shuffle_only(int pass) {
-  launch_shuffle_pass(st, in, cs_count + (unsigned long long)nraw, nclust_h, pass, s);
-  launch_report(st, pass, s);
-}
-void Run::launch_round_tail_noshuffle() {
-  launch_p_update(st, in, o->greedy != 0, o->detect_singletons != 0, -1, s);
-  BudParams bp{o->min_fold, o->min_hamming, o->min_abund};
-  launch_bud_scan(st, in, bp, nclust_h, -1, s);
-  launch_report(st, -1, s);
-}
-
-// Owner mode: gather every rank's report, keep the local counters, merge the bud candidates and the move lists so that
-// replay_moves / decide_bud see exactly what a single-GPU run would have reported.  Every rank computes the same merge.
-void Run::sync_report_owner() {
+// Copies every rank's report back (sharded: one all-gather first), keeps the local counters, merges the bud candidates and the
+// move lists so that replay_moves / decide_bud see exactly what a single-GPU run reports.  Every rank computes the same merge.
+void Run::sync_report() {
   const int W = cx->world;
-  const size_t G = RR_PAD + (size_t)eager_sh * 8;                  // per rank: the report and the head of its move list
-  d_gather_all.alloc((size_t)W * G); h_gather_all.alloc((size_t)W * G);
-  NC(g_nccl.AllGather(d_repmv.p, d_gather_all.p, G, ncclChar, cx->comm, s));
-  d2h_pinned(h_gather_all.p, d_gather_all.p, (size_t)W * G);
+  const size_t G = RR_PAD + (size_t)eager * 8;                     // per rank: the report and the head of its move list
+  const uint8_t *gathered = d_repmv.p;
+  if (W > 1) {
+    d_gather_all.alloc((size_t)W * G);
+    NC(g_nccl.AllGather(d_repmv.p, d_gather_all.p, G, ncclChar, cx->comm, s));
+    gathered = d_gather_all.p;
+  }
+  h_gather_all.alloc((size_t)W * G);
+  d2h_pinned(h_gather_all.p, gathered, (size_t)W * G);
   sync();
   rep_all.resize(W);
   for (int q = 0; q < W; q++) rep_all[q] = (const RoundReport *)(h_gather_all.p + (size_t)q * G);
@@ -1064,14 +1026,17 @@ void Run::sync_report_owner() {
   if (maxM) {
     const uint32_t *src = (const uint32_t *)(h_gather_all.p + RR_PAD);      // rank q's moves: src + q * stride (u32 units)
     size_t stride = G / 4;
-    if (maxM > eager_sh) {     // a round that moved more than the report's gather carries: the whole lists, padded to the longest one
-      if ((size_t)W * maxM * 2 > d_moves_all.cap || !d_moves_all.p) {     // grown in powers of two and kept across runs: allocation calls stall behind the kernel driver's lock
-        size_t m = 65536;
-        while (m < maxM) m *= 2;
-        d_moves_all.alloc((size_t)W * m * 2); h_moves_all.alloc((size_t)W * m * 2);
+    if (maxM > eager) {        // a round that moved more than the report's copy carries: the whole lists, padded to the longest one
+      size_t m = 65536;                // grown in powers of two and kept across runs: allocation calls stall behind the kernel driver's lock
+      while (m < maxM) m *= 2;
+      if (W > 1 && (size_t)W * maxM * 2 > d_moves_all.cap) d_moves_all.alloc((size_t)W * m * 2);
+      if ((size_t)W * maxM * 2 > h_moves_all.cap) h_moves_all.alloc((size_t)W * m * 2);
+      const uint32_t *lists = st.moves;
+      if (W > 1) {
+        NC(g_nccl.AllGather(st.moves, d_moves_all.p, (size_t)maxM * 8, ncclChar, cx->comm, s));
+        lists = d_moves_all.p;
       }
-      NC(g_nccl.AllGather(mv_dev, d_moves_all.p, (size_t)maxM * 8, ncclChar, cx->comm, s));
-      d2h_pinned(h_moves_all.p, d_moves_all.p, (size_t)W * maxM * 8);
+      d2h_pinned(h_moves_all.p, lists, (size_t)W * maxM * 8);
       sync();
       src = h_moves_all.p; stride = (size_t)maxM * 2;
     }
@@ -1114,25 +1079,6 @@ void Run::sync_report_owner() {
     }
   }
   h_report->ctr[CTR_NTIE] = nt; h_report->ctr[CTR_NTIE_PR] = ntp;
-}
-
-void Run::sync_report() {
-  if (owner) { sync_report_owner(); return; }
-  d2h_pinned(h_report, rep_dev, sizeof(RoundReport));
-  const unsigned eager = std::min<unsigned>(MOVES_EAGER, move_cap);
-  d2h_pinned(h_moves, mv_dev, (size_t)eager * 8);
-  sync();
-  if (h_report->ctr[CTR_NMOVE] > eager && h_report->ctr[CTR_NMOVE] <= move_cap) {
-    d2h_pinned(h_moves + 2 * (size_t)eager, mv_dev + 2 * (size_t)eager, (size_t)(h_report->ctr[CTR_NMOVE] - eager) * 8);
-    sync();
-  }
-  memcpy(h_ctr.p, h_report->ctr, sizeof(unsigned long long) * CTR_N);
-  check_dev_error();
-  cs_count = h_report->ctr[CTR_CS_COUNT];
-  if (count_round) { tot_nw += h_report->ctr[CTR_NW]; tot_gl += h_report->ctr[CTR_GL]; count_round = false; }
-  est_active = std::max<unsigned long long>(1024, 2 * h_report->ctr[CTR_NW]);
-  if (cs_count > st.cs_cap) throw Err{"dada2b: comparison store overflow"};
-  if (h_report->ctr[CTR_NMOVE] > move_cap) throw Err{"dada2b: move list overflow"};
 }
 
 // b_shuffle2's container updates (cluster.cpp:242-260) replayed on the host member arrays in the
@@ -1238,8 +1184,9 @@ int Run::decide_bud(uint32_t *r_out, uint32_t *from_out) {
   unsigned long long nt = R.ctr[CTR_NTIE], ntp = R.ctr[CTR_NTIE_PR];
   std::vector<uint32_t> big, bigp;
   const uint32_t *tr = R.tie_r, *trp = R.tiep_r;
-  if (owner && (nt > TIE_MAX || ntp > TIE_MAX)) {
-    // every rank lists its own candidates at the global optimum; the lists are exchanged padded to the longest one
+  if (nt > TIE_MAX || ntp > TIE_MAX) {
+    // pathological tie set: every rank lists its own candidates at the global optimum; sharded, the lists are exchanged padded
+    // to the longest one
     const int W = cx->world;
     struct RepView { const std::vector<const RoundReport *> &v; const RoundReport &operator[](int q) const { return *v[q]; } } rep{rep_all};
     std::vector<unsigned long long> na(W, 0), np(W, 0);
@@ -1250,16 +1197,21 @@ int Run::decide_bud(uint32_t *r_out, uint32_t *from_out) {
       maxn = std::max(maxn, std::max(na[q], np[q]));
     }
     DBuf<uint32_t> &d1 = tie_d1, &d2 = tie_d2, &g1 = tie_g1, &g2 = tie_g2;       // members: no cudaMalloc / cudaFree in a steady-state pass
-    d1.alloc(maxn); d2.alloc(maxn); g1.alloc(maxn * W); g2.alloc(maxn * W);
+    d1.alloc(maxn); d2.alloc(maxn);
     unsigned long long gl[6] = {R.ctr[CTR_PMIN], R.ctr[CTR_RMAX], 0ull, R.ctr[CTR_PMIN_PR], R.ctr[CTR_RMAX_PR], 0ull};
     static_assert(CTR_RMAX == CTR_PMIN + 1 && CTR_NTIE == CTR_PMIN + 2 && CTR_PMIN_PR == CTR_PMIN + 3 && CTR_NTIE_PR == CTR_PMIN + 5, "counter layout");
     h2d(ctr.p + CTR_PMIN, gl, sizeof(gl));
     BudParams bp{o->min_fold, o->min_hamming, o->min_abund};
     launch_bud_collect_owned(st, in, ts, bp, d1.p, d2.p, (unsigned)maxn, s);
-    NC(g_nccl.AllGather(d1.p, g1.p, (size_t)maxn * 4, ncclChar, cx->comm, s));
-    NC(g_nccl.AllGather(d2.p, g2.p, (size_t)maxn * 4, ncclChar, cx->comm, s));
+    const uint32_t *all1 = d1.p, *all2 = d2.p;
+    if (W > 1) {
+      g1.alloc(maxn * W); g2.alloc(maxn * W);
+      NC(g_nccl.AllGather(d1.p, g1.p, (size_t)maxn * 4, ncclChar, cx->comm, s));
+      NC(g_nccl.AllGather(d2.p, g2.p, (size_t)maxn * 4, ncclChar, cx->comm, s));
+      all1 = g1.p; all2 = g2.p;
+    }
     std::vector<uint32_t> h1(maxn * W), h2(maxn * W);
-    d2h(h1.data(), g1.p, h1.size() * 4); d2h(h2.data(), g2.p, h2.size() * 4);
+    d2h(h1.data(), all1, h1.size() * 4); d2h(h2.data(), all2, h2.size() * 4);
     sync();
     for (int q = 0; q < W; q++) {
       big.insert(big.end(), h1.begin() + (size_t)q * maxn, h1.begin() + (size_t)q * maxn + na[q]);
@@ -1267,20 +1219,8 @@ int Run::decide_bud(uint32_t *r_out, uint32_t *from_out) {
     }
     if (big.size() != nt || bigp.size() != ntp) throw Err{"dada2b: inconsistent tie lists across ranks"};
     tr = big.data(); trp = bigp.data();
-  } else if (nt > TIE_MAX || ntp > TIE_MAX) {                          // pathological tie set: fetch all of it
-    const unsigned cap = (unsigned)std::max(nt, ntp);
-    DBuf<uint32_t> &d1 = tie_d1, &d2 = tie_d2; d1.alloc(cap); d2.alloc(cap);
-    unsigned long long z[2] = {0ull, 0ull};
-    h2d(ctr.p + CTR_NTIE, &z[0], 8); h2d(ctr.p + CTR_NTIE_PR, &z[1], 8);
-    BudParams bp{o->min_fold, o->min_hamming, o->min_abund};
-    launch_bud_collect_big(st, in, bp, d1.p, d2.p, cap, s);
-    big.resize(nt); bigp.resize(ntp);
-    if (nt) d2h(big.data(), d1.p, nt * 4);
-    if (ntp) d2h(bigp.data(), d2.p, ntp * 4);
-    sync();
-    tr = big.data(); trp = bigp.data();
   }
-  // The device reported the cluster and the cluster's reads of every listed candidate (fused tail): a single candidate needs nothing
+  // The device reported the cluster and the cluster's reads of every listed candidate: a single candidate needs nothing
   // from the host's member arrays, so the replay worker may still be busy with this round's moves.  Exact ties do: wait for it.
   const bool from_report = async_replay && nt <= 1 && ntp <= 1;
   if (!from_report) drain_replay();
@@ -1322,20 +1262,17 @@ int Run::decide_bud(uint32_t *r_out, uint32_t *from_out) {
     if (R.tie_r[k] == r && type == 'A') { lam = R.tie_lam[k]; ham = R.tie_ham[k]; have = true; }
   for (unsigned long long k = 0; k < std::min<unsigned long long>(ntp, TIE_MAX) && !have; k++)
     if (R.tiep_r[k] == r && type == 'P') { lam = R.tiep_lam[k]; ham = R.tiep_ham[k]; have = true; }
-  if (!have && owner) {            // only the winner's owner holds its comparison: sum all-reduce of (lambda bits, hamming) with zeros elsewhere
+  if (!have) {            // only the winner's owner holds its comparison: sum all-reduce of (lambda bits, hamming) with zeros elsewhere
     DBuf<unsigned long long> &w2 = win_buf; w2.alloc(2); w2.zero(s);
     if ((int)(r % (uint32_t)cx->world) == cx->rank) {
       CK(cudaMemcpyAsync(w2.p, comp_lambda.p + r, 8, cudaMemcpyDeviceToDevice, s));
       CK(cudaMemcpyAsync(w2.p + 1, comp_ham.p + r, 4, cudaMemcpyDeviceToDevice, s));
     }
-    NC(g_nccl.AllReduce(w2.p, w2.p, 2, ncclUint64, ncclSum, cx->comm, s));
+    if (cx->world > 1) NC(g_nccl.AllReduce(w2.p, w2.p, 2, ncclUint64, ncclSum, cx->comm, s));
     unsigned long long hw[2];
     d2h(hw, w2.p, 16);
     sync();
     memcpy(&lam, &hw[0], 8); ham = (uint32_t)hw[1];
-  } else if (!have) {
-    d2h(&lam, comp_lambda.p + r, 8); d2h(&ham, comp_ham.p + r, 4);
-    sync();
   }
   const double expected = lam * (double)from_reads;
   const uint32_t ni = (uint32_t)nclust_h;                       // b_add_bi + bi_add_raw + bi_assign_center
@@ -1412,11 +1349,10 @@ void Run::finish(dada2b_out *out) {
     NC(g_nccl.AllReduce(cq_sum.p, cq_sum.p, (size_t)nclust * maxlen, ncclUint64, ncclSum, cx->comm, s));
     NC(g_nccl.AllReduce(cq_cnt.p, cq_cnt.p, (size_t)nclust * maxlen, ncclUint64, ncclSum, cx->comm, s));
     NC(g_nccl.AllReduce(nsubs_final.p, nsubs_final.p, (size_t)nraw, ncclUint32, ncclSum, cx->comm, s));
-    if (owner) {       // final p / correct are only meaningful on a raw's owner: zero the rest, then the sum is the full array
-      launch_mask_unowned(this->p.p, correct.p, nraw, cx->rank, cx->world, s);
-      NC(g_nccl.AllReduce(this->p.p, this->p.p, (size_t)nraw, ncclFloat64, ncclSum, cx->comm, s));
-      NC(g_nccl.AllReduce(correct.p, correct.p, (size_t)nraw, ncclUint8, ncclSum, cx->comm, s));
-    }
+    // final p / correct are only meaningful on a raw's owner: zero the rest, then the sum is the full array
+    launch_mask_unowned(this->p.p, correct.p, nraw, cx->rank, cx->world, s);
+    NC(g_nccl.AllReduce(this->p.p, this->p.p, (size_t)nraw, ncclFloat64, ncclSum, cx->comm, s));
+    NC(g_nccl.AllReduce(correct.p, correct.p, (size_t)nraw, ncclUint8, ncclSum, cx->comm, s));
   }
   // birth subs: sub_new(centre of birth_comp.i, centre i, use_kmers, cutoff 1.0)   Rmain.cpp:206-209
   const uint32_t npair = nclust - 1;
@@ -1478,14 +1414,13 @@ void Run::finish(dada2b_out *out) {
     DBuf<unsigned long long> &dcount = fin_dcount; dcount.alloc(1);
     for (;;) {
       trip_ij.alloc((size_t)cap * 2); trip_v.alloc(cap); dcount.zero(s);
-      if (owner) launch_posthoc_owned(st, nraw, cs_count, center_cluster.p, trip_ij.p, trip_v.p, cap, dcount.p, cx->rank, cx->world, s);
-      else launch_posthoc(st, nraw, cs_count, center_cluster.p, trip_ij.p, trip_v.p, cap, dcount.p, s);
+      launch_posthoc_owned(st, nraw, cs_count, center_cluster.p, trip_ij.p, trip_v.p, cap, dcount.p, cx->rank, cx->world, s);
       d2h(&cnt, dcount.p, 8);
       sync();
       if (cnt <= cap) break;
       cap = (unsigned)cnt + 16;
     }
-    if (owner) {       // every rank found the triples of the centres it owns: exchange them (counts first, then padded payloads)
+    if (cx->world > 1) {       // every rank found the triples of the centres it owns: exchange them (counts first, then padded payloads)
       const int W = cx->world;
       DBuf<unsigned long long> &dall = fin_dall; dall.alloc(W);
       NC(g_nccl.AllGather(dcount.p, dall.p, 1, ncclUint64, cx->comm, s));
@@ -1714,14 +1649,14 @@ dada2b_out *do_run(dada2b_ctx *cx, const double *err_cm, int Q, const dada2b_opt
     const uint8_t one = 1;
     R.h2d(R.is_center.p + c0, &one, 1);
     R.h2d(R.slot0.p + 0, &one, 1);
-    R.h2d(R.cl_reads.p, &cx->total_reads, 4); R.h2d(R.cl_reads_next.p, &cx->total_reads, 4);
+    R.h2d(R.cl_reads.p, &cx->total_reads, 4);
     R.h2d(R.cl_center.p, &c0, 4);
     R.h2d(R.cl_update_e.p, &one, 1); R.h2d(R.cl_check_locks.p, &one, 1);
     R.sync();
   }
-  // host bookkeeping off the critical path (see Run::ReplayEvent): needs the fused tail's report fields and every cluster's centre at
-  // slot 0 (abundance-sorted input, what derepFastq produces); DADA2B_SYNC_REPLAY is a test hook
-  R.async_replay = R.fused_tail && c0 == 0 && getenv("DADA2B_SYNC_REPLAY") == nullptr;
+  // host bookkeeping off the critical path (see Run::ReplayEvent): needs every cluster's centre at slot 0 (abundance-sorted input,
+  // what derepFastq produces); DADA2B_SYNC_REPLAY is a test hook
+  R.async_replay = c0 == 0 && getenv("DADA2B_SYNC_REPLAY") == nullptr;
   TDBG("cluster 0 initialised");
   const double t1 = now_ms();
   const bool dbg = o->verbose || getenv("DADA2B_VERBOSE");
@@ -1747,23 +1682,11 @@ dada2b_out *do_run(dada2b_ctx *cx, const double *err_cm, int Q, const dada2b_opt
     int last = R.NP - 1;
     int ran = R.replay_moves(0, last);
     h_enq += te - tr; h_wait += tw - te; h_replay += now_ms() - tw;
-    if (!R.h_report->converged && R.fused_tail) {     // rare: more than NP passes needed: one more fused pass at a time
-      while (!R.h_report->converged && last + 1 < MAX_PASS) {
-        last++;
-        R.launch_round_tail(last, 1);        // at pass MAX_SHUFFLE - 1 the tail proceeds regardless (dada.h:30, Rmain.cpp:322-325)
-        R.sync_report();
-        ran += R.replay_moves(last, last);
-      }
-    } else if (!R.h_report->converged) {     // rare: more than NP passes needed (MAX_SHUFFLE = 10, dada.h:30)
-      while (last + 1 < MAX_PASS) {
-        last++;
-        R.launch_shuffle_only(last);
-        R.sync_report();
-        ran += R.replay_moves(last, last);
-        if (R.h_report->converged) break;
-      }
-      R.launch_round_tail_noshuffle();       // p-update + bud scan skipped themselves on the device: run them now
+    while (!R.h_report->converged && last + 1 < MAX_PASS) {      // rare: more than NP passes needed: one more pass at a time
+      last++;
+      R.launch_round_tail(last, 1);          // at pass MAX_SHUFFLE - 1 the tail proceeds regardless (dada.h:30, Rmain.cpp:322-325)
       R.sync_report();
+      ran += R.replay_moves(last, last);
     }
     R.n_rounds++;
     if (dbg) fprintf(stderr, "[dada2b] C%d seed=%u: round %.3f ms (%d passes), cs=%llu nw=%llu gl=%llu moves=%llu\n", newi,

@@ -6,10 +6,8 @@
 //                       nwalign_vectorized.cpp:71-318, pval.cpp:144-197, cluster.cpp:90-204
 // k_align<FINAL>        FinalSubsParallel + transition / quality matrices   Rmain.cpp:179-236, error.cpp:131-172,225-258
 // k_align<BIRTH>        birth subs                                          Rmain.cpp:206-209, error.cpp:261-300
-// k_shuffle_*           b_shuffle2                                          cluster.cpp:210-266
-// k_p_update            b_p_update / get_pA / calc_pA                       pval.cpp:14-89
-// k_bud_*               b_bud's arg-min scan                                cluster.cpp:274-308
 // k_final_p             final p / correct flag                              Rmain.cpp:239-252
+// (b_shuffle2 / b_p_update / b_bud: the round tail of dd_round2.cu)
 //
 // Integer DP + scalar fp64: no tensor cores by construction (SURVEY.md 8d).
 #include "dd_common.h"
@@ -323,21 +321,6 @@ __global__ void k_calc_pA_vec(const int *reads, const double *E, const int *prio
   if (x < n) out[x] = calc_pA(reads[x], E[x], prior[x] != 0);
 }
 
-// Post-hoc expected reads (error.cpp:106-116): every stored comparison whose raw is the centre of
-// another cluster j contributes lambda * reads_i to tot_e[j]; emit (i, j, value) triples, the host adds
-// them in ascending i like the reference's cluster-order loop.
-__global__ void k_posthoc(DevState st, unsigned long long n, const int *center_cluster, uint32_t *trip_ij, double *trip_v,
-                          unsigned cap, unsigned long long *count) {
-  unsigned long long x = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
-  if (x >= n) return;
-  const int j = center_cluster[st.cs_index[x]];
-  if (j < 0) return;
-  const uint32_t i = st.cs_i[x];
-  if ((int)i == j) return;
-  unsigned long long s = atomicAdd(count, 1ull);
-  if (s < cap) { trip_ij[2 * s] = i; trip_ij[2 * s + 1] = (uint32_t)j; trip_v[s] = st.cs_lambda[x] * (double)st.cl_reads[i]; }
-}
-
 // ------------------------------- launch wrappers --------------------------------------
 // kernel launches of the CALLING thread (a context is driven by one thread at a time, include/dada2b.h: per-run deltas stay
 // exact when several contexts run on several threads, e.g. the ranks of a sharded run inside one process)
@@ -369,13 +352,6 @@ void launch_final_p(const DevState &st, const DevIn &in, double omegaC, cudaStre
 void launch_calc_pA_vec(const int *reads, const double *E, const int *prior, double *out, int n, cudaStream_t s) {
   COUNT_LAUNCH(1);
   k_calc_pA_vec<<<(n + 127) / 128, 128, 0, s>>>(reads, E, prior, out, n);
-}
-void launch_posthoc(const DevState &st, int nraw, unsigned long long n_entries, const int *center_cluster, uint32_t *trip_ij,
-                    double *trip_v, unsigned cap, unsigned long long *count, cudaStream_t s) {
-  (void)nraw;
-  if (!n_entries) return;
-  COUNT_LAUNCH(1);
-  k_posthoc<<<(unsigned)((n_entries + 255) / 256), 256, 0, s>>>(st, n_entries, center_cluster, trip_ij, trip_v, cap, count);
 }
 
 }  // namespace dd2

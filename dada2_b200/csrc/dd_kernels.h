@@ -108,7 +108,7 @@ void launch_classify(const ClassifyArgs &a, int grid, int block, size_t smem, cu
 void launch_align(int mode, const AlignArgs &a, int grid, int block, size_t smem, cudaStream_t s);
 cudaError_t align_set_smem(size_t bytes);
 
-// fused round tail (dd_round2.cu; EXPERIMENTAL, DADA2B_FUSED_TAIL=1)
+// round tail (dd_round2.cu): shuffle passes, p-update, bud scan and report of every round
 struct BlkBest { unsigned long long pb, pbp; uint32_t rd, rdp, n, np; };
 struct TailState {
   uint32_t *head;          // [nraw] newest stored comparison of the raw
@@ -116,18 +116,19 @@ struct TailState {
   int *rows;               // [MAX_PASS][row_stride] per shuffle pass: reads delta per cluster | touched flag per cluster | moves
   uint32_t cl_cap, row_stride;      // row_stride = 2 * cl_cap + 4
   uint32_t *nmove_pass;    // [MAX_PASS] moves THIS rank made in pass k of the current round
-  int rank, world;         // owner mode: this rank shuffles / scans raws r % world == rank only (1 rank: every raw)
+  int rank, world;         // this rank shuffles / scans raws r % world == rank only (1 rank: every raw)
   unsigned *done;          // block tickets of k_tail_final
   BlkBest *blk;            // [grid of k_tail_final] per-block bud minima
   uint32_t *blk_ties, *blk_ties_pr;   // [grid][TIE_MAX] their tie candidates
 };
 struct BudParams;
-bool tail_fits(int nclust);
+// largest cluster count whose per-cluster state the tail kernels can stage in shared memory (smem = true); above it, smem = false
+int tail_smem_clusters_max();
 int tail_grid(int nraw);
 void launch_tail_link(const DevState &st, const TailState &ts, unsigned long long base, uint32_t cluster_i, int nraw, int nclust, cudaStream_t s);
-void launch_tail_pass(const DevState &st, const DevIn &in, const TailState &ts, int pass, int nclust, cudaStream_t s);
+void launch_tail_pass(const DevState &st, const DevIn &in, const TailState &ts, int pass, int nclust, bool smem, cudaStream_t s);
 void launch_tail_final(const DevState &st, const DevIn &in, const TailState &ts, const BudParams &bp, int greedy, int detect_singletons,
-                       int last_pass, int nclust, int mode, cudaStream_t s);
+                       int last_pass, int nclust, int mode, bool smem, cudaStream_t s);
 
 void launch_bud_collect_owned(const DevState &st, const DevIn &in, const TailState &ts, const BudParams &bp, uint32_t *ties, uint32_t *ties_pr,
                               unsigned cap, cudaStream_t s);
@@ -143,16 +144,9 @@ struct BudParams {
   double skip_log = 1e300, skip_log_prior = 1e300;
 };
 void launch_round_begin(const DevState &st, int apply, uint32_t r, uint32_t from, uint32_t newi, uint32_t reads_r, cudaStream_t s);
-void launch_shuffle_pass(const DevState &st, const DevIn &in, unsigned long long n_entries_upper, int nclust, int pass, cudaStream_t s);
-void launch_p_update(const DevState &st, const DevIn &in, int greedy, int detect_singletons, int last_pass, cudaStream_t s);
-void launch_bud_scan(const DevState &st, const DevIn &in, const BudParams &bp, int nclust, int last_pass, cudaStream_t s);
-void launch_report(const DevState &st, int last_pass, cudaStream_t s);
 void launch_fill_f64(double *p, double v, size_t n, cudaStream_t s);
 void launch_center_cluster(int *cc, const uint32_t *cl_center, int nclust, cudaStream_t s);
-void launch_bud_collect_big(const DevState &st, const DevIn &in, const BudParams &bp, uint32_t *ties, uint32_t *ties_pr, unsigned cap, cudaStream_t s);
 void launch_final_p(const DevState &st, const DevIn &in, double omegaC, cudaStream_t s);
 void launch_calc_pA_vec(const int *reads, const double *E, const int *prior, double *out, int n, cudaStream_t s);
-void launch_posthoc(const DevState &st, int nraw, unsigned long long n_entries, const int *center_cluster,
-                    uint32_t *trip_ij, double *trip_v, unsigned cap, unsigned long long *count, cudaStream_t s);
 
 }  // namespace dd2

@@ -1,17 +1,11 @@
-// Per-round control kernels of the divisive loop (product code, sm_90a): everything between two
-// bud decisions runs on the device without host round trips.
+// Control kernels of the divisive loop (product code, sm_90a); the round tail (shuffle, p-update, bud scan, report) is
+// dd_round2.cu.
 //
 //   k_round_begin     b_bud's container updates for the new cluster      cluster.cpp:315-330, containers.cpp:150-197
-//   k_shuffle_*       b_shuffle2                                        cluster.cpp:210-266
-//   k_p_update        b_p_update / get_pA / calc_pA + greedy locks      pval.cpp:14-89
-//   k_bud_*           b_bud's arg-min scan                              cluster.cpp:274-308
-//   k_report          snapshot for the host (mapped pinned memory)
-//
-// The host only replays the (rare) membership moves on its slot-ordered member arrays -- which the
-// reference's tie-breaks depend on -- and picks the bud winner among exact ties.
+//   k_raw_bounds      per-raw factors of the two-phase loop NW's bound
+//   k_qrows_*         quality / sequence rows of a list of raws <-> a dense buffer (sharded uploads, finish())
 #include "dd_common.h"
 #include "dd_kernels.h"
-#include "ppois.cuh"
 
 namespace dd2 {
 
@@ -23,166 +17,14 @@ __global__ void k_round_begin(DevState st, int apply, uint32_t r, uint32_t from,
     if (apply) {   // bi_pop_raw(from) ; b_add_bi ; bi_add_raw ; bi_assign_center
       st.cluster_of[r] = newi; st.is_center[r] = 1; st.slot0[r] = 1; st.lock[r] = 0;
       st.cl_center[newi] = r;
-      st.cl_reads[from] -= reads_r; st.cl_reads_next[from] = st.cl_reads[from];
-      st.cl_reads[newi] = reads_r; st.cl_reads_next[newi] = reads_r;
+      st.cl_reads[from] -= reads_r;
+      st.cl_reads[newi] = reads_r;
       st.cl_update_e[from] = 1; st.cl_update_e[newi] = 1; st.cl_check_locks[newi] = 1;
     }
     st.ctr[CTR_NW] = 0; st.ctr[CTR_GL] = 0; st.ctr[CTR_FB] = 0; st.ctr[CTR_NMOVE] = 0;
     st.ctr[CTR_CAND] = 0; st.ctr[CTR_OLD] = 0; st.ctr[CTR_SURV] = 0; st.ctr[CTR_UNEQ_B] = 0; st.ctr[CTR_UNEQ_X] = 0;   // (no memsets in the round)
   }
   if (threadIdx.x < MAX_PASS + 2) st.pinfo[threadIdx.x] = 0;
-}
-
-// ---- b_shuffle2 ---------------------------------------------------------------------------
-//   max : emax[raw] = max over stored comparisons of lambda * reads(cluster)   (order-preserving
-//         u64 image of the non-negative double; emax is kept zeroed between passes)
-//   arg : best[raw] = lowest entry id attaining emax (entries are appended cluster by cluster, so
-//         lowest id == lowest cluster index == the reference's strict '>' scan, cluster.cpp:229-239)
-//   move: raws whose best cluster differs from the current one move; centres stay (:248-251).
-//         Cluster reads are updated in cl_reads_next so that pass-wide e values use frozen reads.
-__device__ __forceinline__ bool pass_skipped(const DevState &st, int pass) {
-  return pass > 0 && st.pinfo[pass] == st.pinfo[pass - 1];      // previous pass moved nothing
-}
-__global__ void k_shuffle_max(DevState st, int pass) {
-  if (pass_skipped(st, pass)) return;
-  const unsigned long long n = st.ctr[CTR_CS_COUNT];
-  for (unsigned long long x = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; x < n;
-       x += (unsigned long long)gridDim.x * blockDim.x) {
-    const double e = st.cs_lambda[x] * (double)st.cl_reads[st.cs_i[x]];
-    atomicMax(&st.emax_bits[st.cs_index[x]], (unsigned long long)__double_as_longlong(e));
-  }
-}
-__global__ void k_shuffle_arg(DevState st, int pass) {
-  if (pass_skipped(st, pass)) return;
-  const unsigned long long n = st.ctr[CTR_CS_COUNT];
-  for (unsigned long long x = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; x < n;
-       x += (unsigned long long)gridDim.x * blockDim.x) {
-    const double e = st.cs_lambda[x] * (double)st.cl_reads[st.cs_i[x]];
-    const uint32_t r = st.cs_index[x];
-    if ((unsigned long long)__double_as_longlong(e) == st.emax_bits[r]) atomicMin(&st.best_entry[r], (uint32_t)x);
-  }
-}
-__global__ void k_shuffle_move(DevState st, DevIn in, int pass) {
-  if (pass_skipped(st, pass)) return;
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= in.nraw) return;
-  const uint32_t be = st.best_entry[r];
-  st.emax_bits[r] = 0ull; st.best_entry[r] = 0xFFFFFFFFu;        // leave the scratch clean for the next pass
-  if (be == 0xFFFFFFFFu) return;
-  const uint32_t to = st.cs_i[be], from = st.cluster_of[r];
-  if (to != from && !st.is_center[r]) {
-    const unsigned long long s = atomicAdd(&st.ctr[CTR_NMOVE], 1ull);
-    if (s < st.move_cap) { st.moves[2 * s] = (uint32_t)r; st.moves[2 * s + 1] = to; }
-    st.cluster_of[r] = to;
-    st.comp_lambda[r] = st.cs_lambda[be];                         // raw->comp = *compmax (:257)
-    st.comp_ham[r] = st.cs_ham[be];
-    const uint32_t rd = in.reads[r];
-    atomicSub(&st.cl_reads_next[from], rd);
-    atomicAdd(&st.cl_reads_next[to], rd);
-    st.cl_update_e[from] = 1; st.cl_update_e[to] = 1;
-  }
-}
-__global__ void k_shuffle_commit(DevState st, int nclust, int pass) {
-  for (int x = threadIdx.x; x < nclust; x += blockDim.x) st.cl_reads[x] = st.cl_reads_next[x];
-  if (threadIdx.x == 0) st.pinfo[pass + 1] = (uint32_t)st.ctr[CTR_NMOVE];
-}
-
-// ---- b_p_update ---------------------------------------------------------------------------
-__device__ __forceinline__ bool converged_after(const DevState &st, int last_pass) {
-  return st.pinfo[last_pass + 1] == st.pinfo[last_pass];
-}
-__global__ void k_p_update(DevState st, DevIn in, int greedy, int detect_singletons, int last_pass) {
-  if (last_pass >= 0 && !converged_after(st, last_pass)) return;   // more shuffling needed: host takes over
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r == 0) {                                                   // initialise the bud scan
-    st.ctr[CTR_PMIN] = ~0ull; st.ctr[CTR_RMAX] = 0ull; st.ctr[CTR_NTIE] = 0ull;
-    st.ctr[CTR_PMIN_PR] = ~0ull; st.ctr[CTR_RMAX_PR] = 0ull; st.ctr[CTR_NTIE_PR] = 0ull;
-  }
-  if (r >= in.nraw) return;
-  const uint32_t ci = st.cluster_of[r];
-  const uint32_t reads = in.reads[r];
-  const double lambda = st.comp_lambda[r];
-  if (st.cl_update_e[ci]) {                                        // get_pA pval.cpp:67-89
-    const bool prior = in.prior[r] != 0;
-    double pval;
-    if (reads == 1 && !prior && !detect_singletons) pval = 1.;
-    else if (st.comp_ham[r] == 0) pval = 1.;
-    else if (lambda == 0) pval = 0.;
-    else pval = calc_pA((int)reads, lambda * (double)st.cl_reads[ci], prior || detect_singletons);
-    st.p[r] = pval;
-  }
-  if (greedy && st.cl_check_locks[ci]) {                           // pval.cpp:29-38
-    const uint32_t cen = st.cl_center[ci];
-    const double E_reads_center = (double)in.reads[cen] * lambda;
-    if (E_reads_center > (double)reads) st.lock[r] = 1;
-    if ((uint32_t)r == cen) st.lock[r] = 1;
-  }
-}
-
-// ---- b_bud scan: lexicographic minimum of (p asc, reads desc) over eligible raws; every raw
-// attaining it is reported so the host can apply the (cluster, slot) scan-order tie-break.
-__device__ __forceinline__ bool bud_eligible(const DevState &st, const DevIn &in, int r, const BudParams &bp) {
-  if (st.slot0[r]) return false;                                   // r starts at 1 (cluster.cpp:285)
-  const uint32_t reads = in.reads[r];
-  if ((int)reads < bp.min_abund) return false;
-  if ((int)st.comp_ham[r] < bp.min_hamming) return false;
-  if (!(bp.min_fold <= 1 || ((double)reads) >= bp.min_fold * st.comp_lambda[r] * (double)st.cl_reads[st.cluster_of[r]])) return false;
-  return true;
-}
-__global__ void k_bud_pmin(DevState st, DevIn in, BudParams bp, int nclust, int last_pass) {
-  if (last_pass >= 0 && !converged_after(st, last_pass)) return;
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r < nclust) { st.cl_update_e[r] = 0; st.cl_check_locks[r] = 0; }   // flags consumed by k_p_update
-  unsigned long long pb = ~0ull, pbp = ~0ull;
-  if (r < in.nraw && bud_eligible(st, in, r, bp)) {
-    pb = (unsigned long long)__double_as_longlong(st.p[r]);
-    if (in.prior[r]) pbp = pb;
-  }
-#pragma unroll
-  for (int o = 16; o; o >>= 1) {
-    unsigned long long t = __shfl_xor_sync(0xffffffffu, pb, o); pb = t < pb ? t : pb;
-    t = __shfl_xor_sync(0xffffffffu, pbp, o); pbp = t < pbp ? t : pbp;
-  }
-  if ((threadIdx.x & 31) == 0) {
-    if (pb != ~0ull) atomicMin(&st.ctr[CTR_PMIN], pb);
-    if (pbp != ~0ull) atomicMin(&st.ctr[CTR_PMIN_PR], pbp);
-  }
-}
-__global__ void k_bud_rmax(DevState st, DevIn in, BudParams bp, int last_pass) {
-  if (last_pass >= 0 && !converged_after(st, last_pass)) return;
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= in.nraw) return;
-  const unsigned long long pb = (unsigned long long)__double_as_longlong(st.p[r]);
-  const bool a = pb == st.ctr[CTR_PMIN], b = in.prior[r] && pb == st.ctr[CTR_PMIN_PR];
-  if (!(a || b) || !bud_eligible(st, in, r, bp)) return;
-  if (a) atomicMax(&st.ctr[CTR_RMAX], (unsigned long long)in.reads[r]);
-  if (b) atomicMax(&st.ctr[CTR_RMAX_PR], (unsigned long long)in.reads[r]);
-}
-__global__ void k_bud_collect(DevState st, DevIn in, BudParams bp, int last_pass, uint32_t *big_ties, uint32_t *big_ties_pr,
-                              unsigned big_cap) {
-  if (last_pass >= 0 && !converged_after(st, last_pass)) return;
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= in.nraw) return;
-  const unsigned long long pb = (unsigned long long)__double_as_longlong(st.p[r]);
-  const unsigned long long rd = in.reads[r];
-  const bool a = pb == st.ctr[CTR_PMIN] && rd == st.ctr[CTR_RMAX];
-  const bool b = in.prior[r] && pb == st.ctr[CTR_PMIN_PR] && rd == st.ctr[CTR_RMAX_PR];
-  if (!(a || b) || !bud_eligible(st, in, r, bp)) return;
-  if (a) {
-    const unsigned long long s = atomicAdd(&st.ctr[CTR_NTIE], 1ull);
-    if (s < TIE_MAX) { st.report->tie_r[s] = (uint32_t)r; st.report->tie_lam[s] = st.comp_lambda[r]; st.report->tie_ham[s] = st.comp_ham[r]; }
-    if (big_ties && s < big_cap) big_ties[s] = (uint32_t)r;
-  }
-  if (b) {
-    const unsigned long long s = atomicAdd(&st.ctr[CTR_NTIE_PR], 1ull);
-    if (s < TIE_MAX) { st.report->tiep_r[s] = (uint32_t)r; st.report->tiep_lam[s] = st.comp_lambda[r]; st.report->tiep_ham[s] = st.comp_ham[r]; }
-    if (big_ties_pr && s < big_cap) big_ties_pr[s] = (uint32_t)r;
-  }
-}
-__global__ void k_report(DevState st, int last_pass) {
-  if (threadIdx.x < CTR_N) st.report->ctr[threadIdx.x] = st.ctr[threadIdx.x];
-  if (threadIdx.x < MAX_PASS + 2) st.report->pinfo[threadIdx.x] = st.pinfo[threadIdx.x];
-  if (threadIdx.x == 0) st.report->converged = (last_pass < 0 || converged_after(st, last_pass)) ? 1u : 0u;
 }
 
 // Two-phase loop NW: per-raw bound factors.  S_r = product over the raw's positions of its self-transition factor
@@ -257,35 +99,4 @@ void launch_round_begin(const DevState &st, int apply, uint32_t r, uint32_t from
   count_launch(1);
   k_round_begin<<<1, 32, 0, s>>>(st, apply, r, from, newi, reads_r);
 }
-void launch_shuffle_pass(const DevState &st, const DevIn &in, unsigned long long n_entries_upper, int nclust, int pass, cudaStream_t s) {
-  const int B = 256;
-  const unsigned g = (unsigned)std::min<unsigned long long>((n_entries_upper + B - 1) / B, 148ull * 16);
-  count_launch(4);
-  k_shuffle_max<<<g, B, 0, s>>>(st, pass);
-  k_shuffle_arg<<<g, B, 0, s>>>(st, pass);
-  k_shuffle_move<<<(in.nraw + B - 1) / B, B, 0, s>>>(st, in, pass);
-  k_shuffle_commit<<<1, 256, 0, s>>>(st, nclust, pass);
-}
-void launch_p_update(const DevState &st, const DevIn &in, int greedy, int detect_singletons, int last_pass, cudaStream_t s) {
-  count_launch(1);
-  k_p_update<<<(in.nraw + 127) / 128, 128, 0, s>>>(st, in, greedy, detect_singletons, last_pass);
-}
-void launch_bud_scan(const DevState &st, const DevIn &in, const BudParams &bp, int nclust, int last_pass, cudaStream_t s) {
-  const int B = 256, G = (std::max(in.nraw, nclust) + B - 1) / B;
-  count_launch(3);
-  k_bud_pmin<<<G, B, 0, s>>>(st, in, bp, nclust, last_pass);
-  k_bud_rmax<<<G, B, 0, s>>>(st, in, bp, last_pass);
-  k_bud_collect<<<G, B, 0, s>>>(st, in, bp, last_pass, nullptr, nullptr, 0);
-}
-void launch_bud_collect_big(const DevState &st, const DevIn &in, const BudParams &bp, uint32_t *ties, uint32_t *ties_pr, unsigned cap,
-                            cudaStream_t s) {
-  const int B = 256, G = (in.nraw + B - 1) / B;
-  count_launch(1);
-  k_bud_collect<<<G, B, 0, s>>>(st, in, bp, -1, ties, ties_pr, cap);
-}
-void launch_report(const DevState &st, int last_pass, cudaStream_t s) {
-  count_launch(1);
-  k_report<<<1, 64, 0, s>>>(st, last_pass);
-}
-
 }  // namespace dd2

@@ -1,21 +1,21 @@
-// Fused round tail (product code, sm_90a) -- EXPERIMENTAL, selected with DADA2B_FUSED_TAIL=1; checked on the host SIMT
-// emulator of tests/emu, not yet on hardware.  dd_round.cu stays the default.
-//
-// dd_round.cu spends ~17 small launches per round on b_shuffle2 / b_p_update / b_bud (4 per shuffle pass, 5 after).
-// Here the same work is 1 + NP + 1 launches:
+// Round tail (product code, sm_90a): b_shuffle2 / b_p_update / b_bud of every round, in 1 + NP + 1 launches.
 //
 //   k_tail_link    threads the round's new stored comparisons onto per-raw chains (newest first) and clears the scratch
 //   k_tail_pass    one b_shuffle2 pass (cluster.cpp:210-266) in ONE kernel: every raw walks its own chain for the
 //                  arg-max of lambda * reads(cluster); the pass-wide frozen reads (Appendix A.4 of SURVEY.md) are
-//                  rebuilt per block in shared memory as reads_at_round_start + sum of the earlier passes' deltas,
-//                  and a pass only ever adds to its own delta row, so no commit kernel is needed
+//                  reads_at_round_start + sum of the earlier passes' deltas, and a pass only ever adds to its own delta
+//                  row, so no commit kernel is needed
 //   k_tail_final   b_p_update (pval.cpp:14-40) + the b_bud scan (cluster.cpp:274-308) + the report: per-block
 //                  lexicographic (p asc, reads desc) minima with their tie candidates, reduced by the last block to
 //                  finish (ticket counter), which also commits the cluster reads and clears the per-cluster flags
 //
-// Results are identical to dd_round.cu: the arg-max prefers the lowest cluster index among equal e (chain walked from
-// the newest entry with '>='), moves are recorded per pass (the host replays them in the reference's order) and the
-// host still resolves exact (p, reads) ties by (cluster, slot).
+// k_tail_pass / k_tail_final come in two forms.  SMEM = true stages the per-cluster state (frozen reads, update flags) per
+// block in shared memory, which holds it up to ~32 k clusters; SMEM = false reads it from global memory at every use, for
+// any cluster count.  The host picks the form per launch from the round's cluster count.
+//
+// The arg-max prefers the lowest cluster index among equal e (chain walked from the newest entry with '>='), moves are
+// recorded per pass (the host replays them in the reference's order) and the host resolves exact (p, reads) ties by
+// (cluster, slot).
 #include "dd_common.h"
 #include "dd_kernels.h"
 #include "ppois.cuh"
@@ -25,11 +25,11 @@ namespace dd2 {
 constexpr uint32_t CHAIN_END = 0xFFFFFFFFu;
 
 // Per-pass scratch rows (TailState::rows): [delta(cl_cap) | touched(cl_cap) | moves of the pass (1) | pad].  One row is one
-// NCCL all-reduce in owner mode (every rank shuffles its own raws only).
+// NCCL all-reduce in sharded runs (every rank shuffles its own raws only).
 __device__ __forceinline__ int &row_delta(const TailState &ts, int pass, uint32_t c) { return ts.rows[(size_t)pass * ts.row_stride + c]; }
 __device__ __forceinline__ int &row_touched(const TailState &ts, int pass, uint32_t c) { return ts.rows[(size_t)pass * ts.row_stride + ts.cl_cap + c]; }
 __device__ __forceinline__ int &row_nmove(const TailState &ts, int pass) { return ts.rows[(size_t)pass * ts.row_stride + 2 * (size_t)ts.cl_cap]; }
-// the raw handled by global thread `it`: every raw, or this rank's raws only (owner mode)
+// the raw handled by global thread `it`: this rank's raws only (one rank: every raw)
 __device__ __forceinline__ long long tail_raw(const TailState &ts, long long it) { return it * ts.world + ts.rank; }
 
 __global__ void k_tail_link(DevState st, TailState ts, unsigned long long base, uint32_t cluster_i, int nraw, int nclust) {
@@ -53,13 +53,21 @@ __global__ void k_tail_link(DevState st, TailState ts, unsigned long long base, 
   if (t0 == 0) *ts.done = 0;
 }
 
-// reads of every cluster as frozen at the start of shuffle pass `pass` (pass == npasses: after the last one)
+// reads of cluster c as frozen at the start of shuffle pass `pass` (pass == npasses: after the last one).  Valid until
+// k_tail_final commits them to cl_reads: after that, the deltas would be counted twice.
+__device__ __forceinline__ uint32_t frozen_reads(const DevState &st, const TailState &ts, int pass, int c) {
+  int v = (int)st.cl_reads[c];
+  for (int k = 0; k < pass; k++) v += row_delta(ts, k, c);
+  return (uint32_t)v;
+}
+// cluster c needs a p-update: flagged before the round (new cluster / bud) or touched by a move of passes 0..last_pass
+__device__ __forceinline__ bool cluster_updated(const DevState &st, const TailState &ts, int last_pass, int c) {
+  int u = st.cl_update_e[c];
+  for (int k = 0; k <= last_pass; k++) u |= row_touched(ts, k, c);
+  return u != 0;
+}
 __device__ __forceinline__ void stage_reads(const DevState &st, const TailState &ts, int pass, int nclust, uint32_t *s_reads) {
-  for (int c = threadIdx.x; c < nclust; c += blockDim.x) {
-    int v = (int)st.cl_reads[c];
-    for (int k = 0; k < pass; k++) v += row_delta(ts, k, c);
-    s_reads[c] = (uint32_t)v;
-  }
+  for (int c = threadIdx.x; c < nclust; c += blockDim.x) s_reads[c] = frozen_reads(st, ts, pass, c);
   __syncthreads();
 }
 
@@ -67,10 +75,11 @@ __device__ __forceinline__ void stage_reads(const DevState &st, const TailState 
 // previous entry ...), so what one thread can overlap is what counts (one raw per thread: several waves of 2048 threads per SM,
 // each as long as the chain)
 constexpr int TAIL_RPT = 4;
+template <bool SMEM>
 __global__ void k_tail_pass(DevState st, DevIn in, TailState ts, int pass, int nclust) {
-  extern __shared__ uint32_t s_reads[];
+  extern __shared__ uint32_t s_reads[];                               // SMEM: [nclust] frozen reads
   if (pass > 0 && row_nmove(ts, pass - 1) == 0) return;             // previous pass moved nothing (anywhere): b_shuffle2 returned false
-  stage_reads(st, ts, pass, nclust, s_reads);
+  if (SMEM) stage_reads(st, ts, pass, nclust, s_reads);
   int r[TAIL_RPT];
   uint32_t x[TAIL_RPT], best_x[TAIL_RPT];
   double best_e[TAIL_RPT];
@@ -92,7 +101,7 @@ __global__ void k_tail_pass(DevState st, DevIn in, TailState ts, int pass, int n
 #pragma unroll
     for (int u = 0; u < TAIL_RPT; u++)
       if (x[u] != CHAIN_END) {
-        const double e = lam[u] * (double)s_reads[ci[u]];
+        const double e = lam[u] * (double)(SMEM ? s_reads[ci[u]] : frozen_reads(st, ts, pass, ci[u]));
         if (e >= best_e[u]) { best_e[u] = e; best_x[u] = x[u]; }
         x[u] = nx[u];
       }
@@ -136,9 +145,10 @@ __device__ __noinline__ double calc_pA_call(int reads, double E_reads, bool prio
 // mode 0: p-update + bud scan only if the last launched pass moved nothing (anywhere); otherwise just report and leave the
 //         state for further k_tail_pass launches
 // mode 2: MAX_SHUFFLE passes are done: proceed as if converged (Rmain.cpp:322-325 stops shuffling there)
+template <bool SMEM>
 __global__ void k_tail_final(DevState st, DevIn in, TailState ts, BudParams bp, int greedy, int detect_singletons, int last_pass, int nclust,
                              int mode) {
-  extern __shared__ uint32_t s_reads[];                 // [nclust] reads, then [nclust] bytes: cluster needs a p-update
+  extern __shared__ uint32_t s_reads[];                 // SMEM: [nclust] reads, then [nclust] bytes: cluster needs a p-update
   uint8_t *s_upd = (uint8_t *)(s_reads + nclust);
   __shared__ unsigned long long s_pb[32], s_pbp[32];
   __shared__ uint32_t s_rd[32], s_rdp[32];
@@ -146,13 +156,14 @@ __global__ void k_tail_final(DevState st, DevIn in, TailState ts, BudParams bp, 
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nwarp = blockDim.x >> 5;
   const bool moved_nothing = last_pass < 0 || row_nmove(ts, last_pass) == 0;
   const bool converged = moved_nothing || mode == 2;
+  // the cluster state after the last pass; it stays valid in the last block until the commit below
+  auto reads_of = [&](auto c) { return SMEM ? s_reads[c] : frozen_reads(st, ts, last_pass + 1, c); };
+  auto updated = [&](auto c) { return SMEM ? s_upd[c] != 0 : cluster_updated(st, ts, last_pass, c); };
   if (tid == 0) { s_n = 0; s_np = 0; }
-  for (int c = tid; c < nclust; c += blockDim.x) {
-    int u = st.cl_update_e[c];
-    for (int k = 0; k <= last_pass; k++) u |= row_touched(ts, k, c);
-    s_upd[c] = u ? 1 : 0;
-  }
-  stage_reads(st, ts, last_pass + 1, nclust, s_reads);               // also the barrier behind s_n / s_np / s_upd
+  if (SMEM) {
+    for (int c = tid; c < nclust; c += blockDim.x) s_upd[c] = cluster_updated(st, ts, last_pass, c) ? 1 : 0;
+    stage_reads(st, ts, last_pass + 1, nclust, s_reads);             // also the barrier behind s_n / s_np / s_upd
+  } else __syncthreads();
   // TAIL_RPT raws per thread: the per-CTA work around them (staging, five barriers, the block reductions: two thirds of the
   // kernel's instructions with one raw per thread) is paid once per 1024 raws
   int rA[TAIL_RPT];
@@ -172,7 +183,7 @@ __global__ void k_tail_final(DevState st, DevIn in, TailState ts, BudParams bp, 
       const double lambda = st.comp_lambda[r];
       const uint32_t ham = st.comp_ham[r];
       double pval = st.p[r];
-      if (s_upd[ci]) {                                                   // get_pA pval.cpp:67-89
+      if (updated(ci)) {                                                 // get_pA pval.cpp:67-89
         if (rd == 1 && !prior && !detect_singletons) pval = 1.;
         else if (ham == 0) pval = 1.;
         else if (lambda == 0) pval = 0.;
@@ -181,7 +192,7 @@ __global__ void k_tail_final(DevState st, DevIn in, TailState ts, BudParams bp, 
           // p-values of the output are recomputed after the loop (k_final_p).  p >= P(X = reads) = exp(-E) E^reads / reads!  for
           // either normalisation of calc_pA: when that lower bound is already above the threshold (by a factor e), the raw cannot
           // be budded whatever its exact p is, and the bound is stored in its place -- no incomplete-gamma evaluation.
-          const double E = lambda * (double)s_reads[ci];
+          const double E = lambda * (double)reads_of(ci);
           const double lg = -E + (double)rd * log(E) - lgamma((double)rd + 1.0);
           if (lg >= (prior ? bp.skip_log_prior : bp.skip_log)) pval = exp(lg);
           else pval = calc_pA_call((int)rd, E, prior || detect_singletons);
@@ -195,7 +206,7 @@ __global__ void k_tail_final(DevState st, DevIn in, TailState ts, BudParams bp, 
       }
       // b_bud candidate (cluster.cpp:285-294)
       const bool elig = !st.slot0[r] && (int)rd >= bp.min_abund && (int)ham >= bp.min_hamming &&
-                        (bp.min_fold <= 1 || ((double)rd) >= bp.min_fold * lambda * (double)s_reads[ci]);
+                        (bp.min_fold <= 1 || ((double)rd) >= bp.min_fold * lambda * (double)reads_of(ci));
       rdA[u] = rd;
       if (prior) priorm |= 1u << u;
       if (elig) {
@@ -245,8 +256,11 @@ __global__ void k_tail_final(DevState st, DevIn in, TailState ts, BudParams bp, 
   __threadfence();
   const volatile BlkBest *blk = ts.blk;
   const volatile uint32_t *bt = ts.blk_ties, *btp = ts.blk_ties_pr;
-  if (converged)
-    for (int c = tid; c < nclust; c += blockDim.x) { st.cl_reads[c] = s_reads[c]; st.cl_reads_next[c] = s_reads[c]; }
+  if (converged)       // the other blocks read cl_reads before they took their tickets
+    for (int c = tid; c < nclust; c += blockDim.x) st.cl_reads[c] = reads_of(c);
+  // a cluster's reads after the commit: in global memory, cl_reads now holds them (the barriers below make every thread's commit
+  // visible to the block)
+  auto committed_reads = [&](auto c) { return SMEM ? s_reads[c] : st.cl_reads[c]; };
   if (tid == 0) {
     uint32_t acc = 0;                                                  // pinfo[p+1] = moves recorded up to and including pass p
     st.pinfo[0] = 0;
@@ -281,7 +295,7 @@ __global__ void k_tail_final(DevState st, DevIn in, TailState ts, BudParams bp, 
           const uint32_t rr = bt[(size_t)b * TIE_MAX + k];
           st.report->tie_r[at + k] = rr; st.report->tie_lam[at + k] = st.comp_lambda[rr]; st.report->tie_ham[at + k] = st.comp_ham[rr];
           const uint32_t cc = st.cluster_of[rr];
-          st.report->tie_cl[at + k] = cc; st.report->tie_clreads[at + k] = s_reads[cc];
+          st.report->tie_cl[at + k] = cc; st.report->tie_clreads[at + k] = committed_reads(cc);
         }
       }
       if (blk[b].np && blk[b].pbp == gminp && blk[b].rdp == gmaxp) {
@@ -290,7 +304,7 @@ __global__ void k_tail_final(DevState st, DevIn in, TailState ts, BudParams bp, 
           const uint32_t rr = btp[(size_t)b * TIE_MAX + k];
           st.report->tiep_r[at + k] = rr; st.report->tiep_lam[at + k] = st.comp_lambda[rr]; st.report->tiep_ham[at + k] = st.comp_ham[rr];
           const uint32_t cc = st.cluster_of[rr];
-          st.report->tiep_cl[at + k] = cc; st.report->tiep_clreads[at + k] = s_reads[cc];
+          st.report->tiep_cl[at + k] = cc; st.report->tiep_clreads[at + k] = committed_reads(cc);
         }
       }
     }
@@ -309,7 +323,7 @@ __global__ void k_tail_final(DevState st, DevIn in, TailState ts, BudParams bp, 
 }
 
 
-// ---- owner mode helpers (sharded runs where every rank keeps the comparisons / state of its own raws only) ----
+// ---- per-rank helpers: every rank keeps the comparisons / state of its own raws only (one rank: every raw) ----
 // b_bud tie sets larger than TIE_MAX: this rank's candidates at the GLOBAL (p, reads) optimum (ctr[CTR_PMIN..] set by the host).
 __global__ void k_bud_collect_owned(DevState st, DevIn in, TailState ts, BudParams bp, uint32_t *ties, uint32_t *ties_pr, unsigned cap) {
   const long long rl = tail_raw(ts, blockIdx.x * (long long)blockDim.x + threadIdx.x);
@@ -334,7 +348,9 @@ __global__ void k_mask_unowned(double *p, uint8_t *correct, int nraw, int rank, 
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r < nraw && r % world != rank) { p[r] = 0.0; correct[r] = 0; }
 }
-// k_posthoc (error.cpp:101-119) over this rank's own stored comparisons only
+// Post-hoc expected reads (error.cpp:106-116) over this rank's own stored comparisons: every stored comparison whose raw is the
+// centre of another cluster j contributes lambda * reads_i to tot_e[j]; emit (i, j, value) triples, the host adds them in ascending
+// i like the reference's cluster-order loop.
 __global__ void k_posthoc_owned(DevState st, unsigned long long n, const int *center_cluster, uint32_t *trip_ij, double *trip_v, unsigned cap,
                                 unsigned long long *count, int rank, int world, int nraw) {
   const unsigned long long x = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
@@ -352,28 +368,31 @@ __global__ void k_posthoc_owned(DevState st, unsigned long long n, const int *ce
 constexpr int TAIL_BLOCK = 256;
 constexpr size_t TAIL_SMEM_MAX = 160 * 1024;
 
-bool tail_fits(int nclust) { return (size_t)nclust * 5 + 16 <= TAIL_SMEM_MAX; }
+int tail_smem_clusters_max() { return (int)((TAIL_SMEM_MAX - 16) / 5); }     // k_tail_final<true>: nclust * 5 + 16 bytes
 int tail_grid(int nraw) { return std::max(1, (nraw + TAIL_BLOCK - 1) / TAIL_BLOCK); }
 static int tail_grid_owned(const DevIn &in, const TailState &ts) { return tail_grid((in.nraw - ts.rank + ts.world - 1) / ts.world); }
-bool tail_fits(int nclust);
 
 void launch_tail_link(const DevState &st, const TailState &ts, unsigned long long base, uint32_t cluster_i, int nraw, int nclust, cudaStream_t s) {
   count_launch(1);
   const unsigned g = (unsigned)std::min<unsigned long long>(((unsigned long long)nraw + 255) / 256 + 1, 148ull * 8);
   k_tail_link<<<g, 256, 0, s>>>(st, ts, base, cluster_i, nraw, nclust);
 }
-void launch_tail_pass(const DevState &st, const DevIn &in, const TailState &ts, int pass, int nclust, cudaStream_t s) {
+void launch_tail_pass(const DevState &st, const DevIn &in, const TailState &ts, int pass, int nclust, bool smem, cudaStream_t s) {
   static bool attr_set = false;
-  if (!attr_set) { cudaFuncSetAttribute(k_tail_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TAIL_SMEM_MAX); attr_set = true; }
+  if (!attr_set) { cudaFuncSetAttribute(k_tail_pass<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TAIL_SMEM_MAX); attr_set = true; }
   count_launch(1);
-  k_tail_pass<<<(tail_grid_owned(in, ts) + TAIL_RPT - 1) / TAIL_RPT, TAIL_BLOCK, (size_t)nclust * 4, s>>>(st, in, ts, pass, nclust);
+  const unsigned g = (tail_grid_owned(in, ts) + TAIL_RPT - 1) / TAIL_RPT;
+  if (smem) k_tail_pass<true><<<g, TAIL_BLOCK, (size_t)nclust * 4, s>>>(st, in, ts, pass, nclust);
+  else k_tail_pass<false><<<g, TAIL_BLOCK, 0, s>>>(st, in, ts, pass, nclust);
 }
 void launch_tail_final(const DevState &st, const DevIn &in, const TailState &ts, const BudParams &bp, int greedy, int detect_singletons,
-                       int last_pass, int nclust, int mode, cudaStream_t s) {
+                       int last_pass, int nclust, int mode, bool smem, cudaStream_t s) {
   static bool attr_set = false;
-  if (!attr_set) { cudaFuncSetAttribute(k_tail_final, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TAIL_SMEM_MAX); attr_set = true; }
+  if (!attr_set) { cudaFuncSetAttribute(k_tail_final<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TAIL_SMEM_MAX); attr_set = true; }
   count_launch(1);
-  k_tail_final<<<(tail_grid_owned(in, ts) + TAIL_RPT - 1) / TAIL_RPT, TAIL_BLOCK, (size_t)nclust * 5 + 16, s>>>(st, in, ts, bp, greedy, detect_singletons, last_pass, nclust, mode);
+  const unsigned g = (tail_grid_owned(in, ts) + TAIL_RPT - 1) / TAIL_RPT;
+  if (smem) k_tail_final<true><<<g, TAIL_BLOCK, (size_t)nclust * 5 + 16, s>>>(st, in, ts, bp, greedy, detect_singletons, last_pass, nclust, mode);
+  else k_tail_final<false><<<g, TAIL_BLOCK, 0, s>>>(st, in, ts, bp, greedy, detect_singletons, last_pass, nclust, mode);
 }
 
 void launch_bud_collect_owned(const DevState &st, const DevIn &in, const TailState &ts, const BudParams &bp, uint32_t *ties, uint32_t *ties_pr,

@@ -23,7 +23,7 @@ api._LIBPATH = %r; api._LIB = None
 import tests.test_gpu_parity as T
 T.test_pair_corpus_kernels_match_reference()
 for name in %r:
-    T.test_e2e_matches_reference_golden(name)
+    T.test_e2e_matches_reference_golden(name, None)
 T.test_error_paths()
 print('ASAN RUN OK')
 """
@@ -42,7 +42,7 @@ def _preload():
     return None
 
 
-@pytest.mark.parametrize("flags", [{}, {"DADA2B_FALLBACK": "1", "DADA2B_SPLIT_TAIL": "1"}], ids=["default", "fallback_kernels"])
+@pytest.mark.parametrize("flags", [{}, {"DADA2B_FALLBACK": "1", "DADA2B_TAIL_SMEM_CLUSTERS": "0"}], ids=["default", "fallback_kernels"])
 def test_kernels_are_memory_clean_under_asan(flags):
     asan = _preload()
     if asan is None:

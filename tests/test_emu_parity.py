@@ -76,7 +76,7 @@ def test_emu_error_paths(emu):
 
 @pytest.mark.parametrize("name", E2E)
 def test_emu_e2e(emu, name):
-    _gpu_tests().test_e2e_matches_reference_golden(name)
+    _gpu_tests().test_e2e_matches_reference_golden(name, None)
 
 
 @pytest.mark.parametrize("name", ["syn2000_default", "syn700_ragged", "syn800_nogreedy"])
@@ -105,7 +105,7 @@ def test_emu_e2e_fallback_kernels(emu, monkeypatch, name):
     """DADA2B_FALLBACK=1: no thread-per-pair / lane kernels, no streaming screen -- the general kernels alone (the path of
     ragged lengths, other bands, homopolymer gap costs) reproduce the goldens on every case."""
     monkeypatch.setenv("DADA2B_FALLBACK", "1")
-    _gpu_tests().test_e2e_matches_reference_golden(name)
+    _gpu_tests().test_e2e_matches_reference_golden(name, None)
     assert emu.cuemu_launches(b"k_nwrow<") == 0 and emu.cuemu_launches(b"k_nwlane<") == 0 and emu.cuemu_launches(b"k_prescreen") == 0
 
 
@@ -116,7 +116,7 @@ def test_emu_e2e_every_round_size_class(emu, monkeypatch, name, lane_max):
     small inputs exercise what 1e6-unique runs do: rounds above the threshold (bound pass thread-per-pair, survivors through the
     lane kernel or, above the threshold again, the thread-per-pair exact kernel) and rounds below it (one lane-group launch)."""
     monkeypatch.setenv("DADA2B_LANE_MAX", lane_max)
-    _gpu_tests().test_e2e_matches_reference_golden(name)
+    _gpu_tests().test_e2e_matches_reference_golden(name, None)
     assert emu.cuemu_launches(b"k_nwrow<") > 0
     assert (emu.cuemu_launches(b"k_nwlane<") > 0) == (lane_max != "0")
 
@@ -215,32 +215,38 @@ def test_emu_upload_pipeline_many_blocks(emu, monkeypatch, blk):
 FUSED_E2E = ["syn800_default", "syn800_nogreedy", "syn800_maxclust5", "syn700_ragged"] if not os.environ.get("DADA2B_EMU_FULL") else list(cases.E2E_CASES)
 
 
-@pytest.mark.parametrize("np_passes", [1, 3])
-@pytest.mark.parametrize("name", FUSED_E2E)
-def test_emu_e2e_fused_tail(emu, monkeypatch, name, np_passes):
-    """The fused round tail (dd_round2.cu, the default): 1 + NP + 1 launches instead of ~17 per round.  NP=1
-    makes every round that needs a second shuffle pass continue with one more fused pass at a time."""
+TAIL_CASES = ([pytest.param(name, np_passes, None, id=f"{name}-{np_passes}") for name in FUSED_E2E for np_passes in (1, 3)] +
+              [pytest.param(name, 3, n, id=f"{name}-3-tail_smem{n}") for name in ("syn800_default", "syn700_ragged") for n in ("0", "12")])
+
+
+@pytest.mark.parametrize("name,np_passes,tail_smem", TAIL_CASES)
+def test_emu_e2e_fused_tail(emu, monkeypatch, name, np_passes, tail_smem):
+    """The round tail (dd_round2.cu): 1 + NP + 1 launches per round.  NP=1 makes every round that needs a second shuffle pass
+    continue with one more pass at a time.  DADA2B_TAIL_SMEM_CLUSTERS (test hook) moves the cluster count above which the tail
+    reads its per-cluster state from global memory instead of staging it in shared memory: 0 = every round, 12 = from mid-run on,
+    as runs past ~32 k clusters do."""
     if np_passes == 1 and name not in ("syn800_default", "syn800_maxclust5") and not os.environ.get("DADA2B_EMU_FULL"):
         pytest.skip("quick subset")
     monkeypatch.setenv("DADA2B_NP", str(np_passes))
-    _gpu_tests().test_e2e_matches_reference_golden(name)
+    _gpu_tests().test_e2e_matches_reference_golden(name, tail_smem)
     assert emu.cuemu_launches(b"k_tail_final") > 0
-    assert emu.cuemu_launches(b"k_shuffle_max") == 0 and emu.cuemu_launches(b"k_p_update") == 0
-    if np_passes == 1:      # rounds that moved raws in pass 0 continue with one more fused pass (and final) at a time
+    assert (emu.cuemu_launches(b"k_tail_final<true>") > 0) == (tail_smem != "0")
+    assert (emu.cuemu_launches(b"k_tail_pass<false>") > 0 and emu.cuemu_launches(b"k_tail_final<false>") > 0) == (tail_smem is not None)
+    if np_passes == 1:      # rounds that moved raws in pass 0 continue with one more pass (and final) at a time
         extra = emu.cuemu_launches(b"k_tail_final") - emu.cuemu_launches(b"k_tail_link")
         assert extra >= 0 and (extra > 0 or name not in ("syn800_default", "syn800_maxclust5"))      # e.g. max_clust=1: nothing ever moves
 
 
-@pytest.mark.parametrize("fused", [False, True], ids=["split_tail", "default"])
-def test_emu_large_tie_sets(emu, monkeypatch, fused):
-    """b_bud tie sets larger than TIE_MAX: the host fetches the whole set (k_bud_collect) and applies the scan order."""
+@pytest.mark.parametrize("tail_smem", [None, "0"], ids=["default", "global_tail"])
+def test_emu_large_tie_sets(emu, tail_smem):
+    """b_bud tie sets larger than TIE_MAX: the host fetches the whole set (k_bud_collect_owned) and applies the scan order, with the
+    round tail's per-cluster state in shared memory (default) and in global memory (DADA2B_TAIL_SMEM_CLUSTERS=0)."""
     import tests.test_gpu_zz_ties as TT
-    if not fused:
-        monkeypatch.setenv("DADA2B_SPLIT_TAIL", "1")
     for opts in (dict(), dict(greedy=False), dict(max_clust=30)):
-        TT.test_large_tie_sets_follow_scan_order(opts)
-    assert emu.cuemu_launches(b"k_bud_collect") > 0
-    assert (emu.cuemu_launches(b"k_tail_final") > 0) == fused
+        TT.test_large_tie_sets_follow_scan_order(opts, tail_smem)
+    assert emu.cuemu_launches(b"k_bud_collect_owned") > 0
+    assert (emu.cuemu_launches(b"k_tail_final<false>") > 0) == (tail_smem is not None)
+    assert (emu.cuemu_launches(b"k_tail_final<true>") > 0) == (tail_smem is None)
 
 
 @pytest.mark.parametrize("fallback", [False, True], ids=lambda e: "fallback" if e else "default")
@@ -254,23 +260,31 @@ def test_emu_edge_cases(emu, monkeypatch, fallback):
         cases.check_edge_case(case, dada2_b200.dada_uniques)
 
 
-@pytest.mark.parametrize("world,name", [(2, "syn800_default"), (3, "syn700_ragged"), (8, "syn800_nogreedy")])
-def test_emu_sharded_owner_mode(emu, monkeypatch, world, name):
-    """Owner mode (the default of sharded runs): every rank keeps the stored comparisons and runs shuffle /
+@pytest.mark.parametrize("world,name,tail_smem", [(2, "syn800_default", None), (3, "syn700_ragged", None), (8, "syn800_nogreedy", None),
+                                                  (2, "syn800_default", "0"), (3, "syn700_ragged", "12")],
+                         ids=["2-syn800_default", "3-syn700_ragged", "8-syn800_nogreedy", "2-syn800_default-tail_smem0", "3-syn700_ragged-tail_smem12"])
+def test_emu_sharded_owner_mode(emu, monkeypatch, world, name, tail_smem):
+    """Owner mode (how sharded runs work): every rank keeps the stored comparisons and runs shuffle /
     p-update / bud scan for its own raws only; per pass one all-reduce of the cluster read deltas, per round one
-    all-gather of the ranks' reports and (when raws moved) of the move lists.  No exchange of comparisons at all."""
+    all-gather of the ranks' reports and (when raws moved) of the move lists.  No exchange of comparisons at all.
+    DADA2B_TAIL_SMEM_CLUSTERS: the round tail's per-cluster state in global memory from the first round (0) or from mid-run (12)."""
+    if tail_smem is not None:
+        monkeypatch.setenv("DADA2B_TAIL_SMEM_CLUSTERS", tail_smem)
     _run_sharded(world, name)
     assert emu.cuemu_launches(b"k_cs_append") == 0 and emu.cuemu_launches(b"k_posthoc_owned") > 0
+    assert (emu.cuemu_launches(b"k_tail_final<false>") > 0) == (tail_smem is not None)
 
 
 @pytest.mark.parametrize("eager", [0, 3])
 def test_emu_sharded_report_gather_carries_the_head_of_the_move_lists(emu, monkeypatch, eager):
-    """Owner mode: the round's all-gather carries every rank's report AND the first DADA2B_MOVES_EAGER (test hook; default 1024)
-    moves of its list; only rounds in which some rank moved more exchange the whole lists in a second all-gather.  0: always the
-    second exchange; 3: rounds of both kinds (the default never needs it at this size: every other sharded test)."""
+    """The round's all-gather carries every rank's report AND the first DADA2B_MOVES_EAGER (test hook; default 1024 sharded, 8192 on
+    one GPU) moves of its list; only rounds in which some rank moved more exchange the whole lists in a second all-gather.  0: always
+    the second exchange; 3: rounds of both kinds (the default never needs it at this size: every other test).  World 1 is the same
+    path with a device-to-host copy in place of each all-gather."""
     monkeypatch.setenv("DADA2B_MOVES_EAGER", str(eager))
     _run_sharded(3, "syn800_nogreedy")
     _run_sharded(2, "syn700_ragged", reupload=True)
+    _run_sharded(1, "syn800_default")
 
 
 def test_emu_sharded_owner_mode_ties_and_extra_passes(emu, monkeypatch):

@@ -60,7 +60,7 @@ def test_real_kernels_are_schedule_invariant(sched):
         "import dada2_b200.api as api\n"
         "api._LIBPATH = %r; api._LIB = None\n"
         "import tests.test_gpu_parity as T\n"
-        "T.test_e2e_matches_reference_golden('syn800_default')\n"
+        "T.test_e2e_matches_reference_golden('syn800_default', None)\n"
         "T.test_pair_corpus_kernels_match_reference()\n"
         "print('SCHED OK')\n") % (os.path.dirname(HERE), lib)
     env = dict(os.environ, CUEMU_SCHED=str(sched))

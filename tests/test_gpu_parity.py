@@ -150,11 +150,18 @@ def test_config1_bit_identical():
     assert (got["stats"]["n_align"], got["stats"]["n_shroud"]) == (8655, 3032)          # the oracle's counts (tests/test_oracle.py)
 
 
-@pytest.mark.parametrize("name", sorted(cases.E2E_CASES))
-def test_e2e_matches_reference_golden(name):
+@pytest.mark.parametrize("name,tail_smem", [pytest.param(name, None, id=name) for name in sorted(cases.E2E_CASES)] +
+                         [pytest.param(name, n, id=f"{name}-tail_smem{n}") for name in ("syn800_default", "syn700_ragged", "syn800_priors")
+                          for n in ("0", "12")])
+def test_e2e_matches_reference_golden(name, tail_smem):
+    """tail_smem: DADA2B_TAIL_SMEM_CLUSTERS (test hook), the round tail's per-cluster state in global memory from the first round (0)
+    or from mid-run (12), as runs past ~32 k clusters do."""
     api = _api()
     seqs, ab, pri, err, q, opts = cases.build_case(name)
-    got = api.dada_uniques(seqs, ab, pri, err, q, **opts)
+    with pytest.MonkeyPatch.context() as mp:
+        if tail_smem is not None:
+            mp.setenv("DADA2B_TAIL_SMEM_CLUSTERS", tail_smem)
+        got = api.dada_uniques(seqs, ab, pri, err, q, **opts)
     _check_e2e(name, got)
 
 

@@ -1,6 +1,7 @@
 """Test tooling: the sharded (owner-mode) paths of the emulated library under AddressSanitizer -- report / move-list gather at
-DADA2B_MOVES_EAGER = 0 / 3 / default, sharded re-upload with small packing blocks (tests/test_emu_asan.py covers the unsharded
-kernels inside the suite; this run takes another minute).      python tools/asan_sharded.py"""
+DADA2B_MOVES_EAGER = 0 / 3 / default (world 1 included), sharded re-upload with small packing blocks, the round tail's global-memory
+form from mid-run (tests/test_emu_asan.py covers the unsharded kernels inside the suite; this run takes another minute).
+    python tools/asan_sharded.py"""
 import os
 import subprocess
 import sys
@@ -18,8 +19,11 @@ for eager in ('0', '3', '1024'):
     os.environ['DADA2B_MOVES_EAGER'] = eager
     T._run_sharded(3, 'syn800_nogreedy')
     T._run_sharded(2, 'syn700_ragged', reupload=True)
+    T._run_sharded(1, 'syn800_default')
 os.environ['DADA2B_PACK_BLK'] = '7'
 T._run_sharded(3, 'syn700_ragged', reupload=True)
+os.environ['DADA2B_TAIL_SMEM_CLUSTERS'] = '12'
+T._run_sharded(2, 'syn800_default')
 print('ASAN SHARD OK')
 """
 

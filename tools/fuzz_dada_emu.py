@@ -72,12 +72,15 @@ while time.time() < t_end:
     if (opts["detect_singletons"] or opts["omegaA"] >= 1e-10) and opts["max_clust"] == 0 and len(seqs) > 400:
         opts["max_clust"] = 25                  # permissive thresholds bud hundreds of clusters: bound the emulated rounds
     os.environ["DADA2B_LANE_MAX"] = str(int(rng.choice([0, 32, 256, 16384])))
-    eag = int(rng.choice([-1, -1, 0, 5, 64]))   # sharded runs: moves carried by the report's all-gather (-1: the default, 1024)
+    eag = int(rng.choice([-1, -1, 0, 5, 64]))   # moves carried by the round's report copy (-1: the default, 8192 / 1024 sharded)
     if eag >= 0: os.environ["DADA2B_MOVES_EAGER"] = str(eag)
     else: os.environ.pop("DADA2B_MOVES_EAGER", None)
     blk = int(rng.choice([0, 0, 1, 13, 64]))    # upload pipeline: raws per packing block (0: the default, one block here)
     if blk: os.environ["DADA2B_PACK_BLK"] = str(blk)
     else: os.environ.pop("DADA2B_PACK_BLK", None)
+    tsm = int(rng.choice([-1, -1, 0, 4, 16]))   # round tail: clusters staged in shared memory (-1: the default, every round here)
+    if tsm >= 0: os.environ["DADA2B_TAIL_SMEM_CLUSTERS"] = str(tsm)
+    else: os.environ.pop("DADA2B_TAIL_SMEM_CLUSTERS", None)
     if it < int(os.environ.get("FUZZ_SKIP_UNTIL", "0")): continue          # replay a campaign up to a given iteration (the draws above are all that matters)
     if os.environ.get("FUZZ_VERBOSE"): print("it", it, "n", len(seqs), "L", L, "nvar", nvar, opts, "lane_max", os.environ["DADA2B_LANE_MAX"], "priors", priors is not None, flush=True)
     want = ref.dada_uniques(seqs, ab, priors, err, q, **dict(dict(homo_gap=opts.get("gap", -8)), **opts))
