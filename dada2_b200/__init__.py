@@ -6,3 +6,4 @@ from . import bimera  # noqa: F401,E402
 from . import merge  # noqa: F401,E402
 from . import derep  # noqa: F401,E402
 from . import errmodel  # noqa: F401,E402
+from . import seqtab  # noqa: F401,E402

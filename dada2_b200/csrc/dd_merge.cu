@@ -8,8 +8,7 @@
 // lives in a per-warp global scratch row), then two lane-parallel passes over the alignment columns -- column masks and
 // end-gap runs for the counts, consensus characters written straight to the output row.  Integer / byte work only.
 #include "../../include/dada2b_merge.h"
-#include "dd_nw_warp.cuh"
-#include "dd_bimera.cuh"
+#include "dd_evalpair.cuh"
 #include "dd_hostutil.h"
 
 #include <algorithm>
@@ -55,35 +54,11 @@ __global__ void __launch_bounds__(128) k_merge_pairs(MergeArgs a) {
     unpack_row(a.sq.seq2 + (size_t)q * a.sq.SW, len1, s1, a.P.homo != 0);     // s1 = forward ASV       (al[0])
     unpack_row(a.sq.seq2 + (size_t)k * a.sq.SW, len2, s2, a.P.homo != 0);     // s2 = rc(reverse ASV)   (al[1])
     const int nops = nw_warp(s1, len1, s2, len2, a.P, H, ptr, opw, &cells_lane, &errflag);
-    // pass 1: column masks (forward order): Q = gap in s1's row, P = gap in s2's row, E = equal bases
-    int i0b = 0, i1b = 0, neq = 0, ngap = 0;
-    const int nch = (nops + 31) >> 5;
-    for (int ch = 0; ch < nch; ch++) {
-      const int col = ch * 32 + lane;
-      int op = 0;
-      if (col < nops) { const int e = nops - 1 - col; op = (opw[e >> 4] >> (2 * (e & 15))) & 3; }
-      const unsigned b0 = __ballot_sync(0xffffffffu, op == 1 || op == 3), b1 = __ballot_sync(0xffffffffu, op == 1 || op == 2);
-      const int i0 = i0b + __popc(b0 & lanemask_lt()), i1 = i1b + __popc(b1 & lanemask_lt());
-      const bool eq = op == 1 && ((s1[i0] ^ s2[i1]) & 3) == 0;
-      const unsigned bq = __ballot_sync(0xffffffffu, op == 2), bp = __ballot_sync(0xffffffffu, op == 3), be = __ballot_sync(0xffffffffu, eq);
-      if (lane == 0) { mQ[ch] = bq; mP[ch] = bp; mE[ch] = be; }
-      neq += __popc(be); ngap += __popc(bq) + __popc(bp);
-      i0b += __popc(b0); i1b += __popc(b1);
-    }
-    if (lane == 0) { mQ[nch] = 0; mP[nch] = 0; mE[nch] = 0; }
-    __syncwarp();
-    // C_eval_pair (evaluate.cpp:73-120): the internal part lies between the leading and the trailing end-gap run
-    const int n = nops;
-    const int leadQ = run_fwd(mQ, 0, n), leadP = run_fwd(mP, 0, n);
-    const int trailQ = run_bwd(mQ, n - 1), trailP = run_bwd(mP, n - 1);
-    const int start = leadQ ? leadQ : leadP, end = n - 1 - (trailQ ? trailQ : trailP);
-    int match = 0, mismatch = 0, indel = 0;
-    if (start <= end) {
-      match = neq;                                           // equal columns never lie in an end-gap run
-      indel = ngap - (leadQ ? leadQ : leadP) - (trailQ ? trailQ : trailP);
-      mismatch = (end - start + 1) - match - indel;
-    }
-    if (lane == 0) { int32_t *o = a.counts + (size_t)jb * 3; o[0] = match; o[1] = mismatch; o[2] = indel; }
+    // pass 1: column masks and C_eval_pair's counts (dd_evalpair.cuh)
+    const EvalPair ev = eval_pair_warp(s1, s2, opw, nops, mQ, mP, mE);
+    const int n = nops, nch = (nops + 31) >> 5, leadQ = ev.leadQ, trailP = ev.trailP;
+    int i0b, i1b;
+    if (lane == 0) { int32_t *o = a.counts + (size_t)jb * 3; o[0] = ev.match; o[1] = ev.mismatch; o[2] = ev.indel; }
     // pass 2: C_pair_consensus (evaluate.cpp:131-174); with trim_overhang the leading columns where s1 has a gap and the
     // trailing columns where s2 has a gap are dropped (:152-160); no other column is a double gap, so the kept range is contiguous
     const int drop_lo = a.trim_overhang ? leadQ : 0, drop_hi = a.trim_overhang ? trailP : 0;
