@@ -9,3 +9,6 @@ from . import errmodel  # noqa: F401,E402
 from . import seqtab  # noqa: F401,E402
 from . import filter  # noqa: F401,E402
 from .filter import filterAndTrim, filter_reads  # noqa: F401,E402
+from . import primer  # noqa: F401,E402
+from .primer import removePrimers, remove_primers_reads  # noqa: F401,E402
+from .errmodel import PacBioErrfun  # noqa: F401,E402

@@ -17,7 +17,7 @@
 //                 reads kept as they are first, then the flipped ones)
 //   k_flt_emit    one warp per survivor: the trimmed window, reverse-complemented where flipped, at its output offset
 #include "../../include/dada2b_filter.h"
-#include "dd_hostutil.h"
+#include "dd_flt.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -29,27 +29,11 @@
 
 namespace dd2 {
 
-constexpr unsigned FULL = 0xffffffffu;
 constexpr int FLT_WARPS = 8;                    // warps per block of the per-read kernels
 
 __device__ __forceinline__ int flt_code(char c) {            // A C G T -> 0..3, anything else 4
   switch (c) { case 'A': return 0; case 'C': return 1; case 'G': return 2; case 'T': return 3; default: return 4; }
 }
-__host__ __device__ __forceinline__ char flt_comp(char c) {  // IUPAC complement (Biostrings' DNA_COMPLEMENT_CODE)
-  switch (c) {
-    case 'A': return 'T'; case 'T': return 'A'; case 'C': return 'G'; case 'G': return 'C';
-    case 'R': return 'Y'; case 'Y': return 'R'; case 'K': return 'M'; case 'M': return 'K';
-    case 'B': return 'V'; case 'V': return 'B'; case 'D': return 'H'; case 'H': return 'D';
-    default: return c;                                        // S W N
-  }
-}
-
-// A read as the stages see it: reverse-complemented (qualities reversed) where orient.fwd flipped it.
-struct FltView {
-  const char *s; const uint8_t *q; int L; bool flip;
-  __device__ char base(int p) const { return flip ? flt_comp(s[L - 1 - p]) : s[p]; }
-  __device__ int qual(int p) const { return flip ? q[L - 1 - p] : q[p]; }
-};
 
 // Open-addressing table of k-mer keys (2 bits per base, base j at bits 2j..2j+1), entry = strand mask << 32 | key.
 __device__ __forceinline__ unsigned flt_find(const unsigned long long *t, int lg, unsigned key) {
@@ -396,7 +380,7 @@ __global__ void __launch_bounds__(FLT_WARPS * 32) k_flt_emit(FltArgs a, const ui
       const long long o = a.in[sm].off[i];
       const FltView v{a.in[sm].seq + o, a.in[sm].qual + o, (int)(a.in[sm].off[i + 1] - o), a.nm == 1 && fp};
       const int s0 = st[m].start, len = st[m].end - st[m].start;
-      for (int j = lane; j < len; j += 32) { out.seq[m][off + j] = v.base(s0 + j); out.qual[m][off + j] = (uint8_t)v.qual(s0 + j); }
+      flt_copy_window(v, s0, len, out.seq[m] + off, out.qual[m] + off, lane);
       if (lane == 0) out.off[m][pos] = (long long)off;
     }
   }
@@ -435,27 +419,21 @@ __global__ void __launch_bounds__(FLT_WARPS * 32) k_flt_cplx(const char *seq, co
 
 using namespace dd2;
 
-namespace {
-
-struct FltScan {                                          // in-place exclusive u64 scans on one stream
-  cudaStream_t s;
-  BBuf<unsigned long long> sums;
-  long long launches = 0;
-  void operator()(unsigned long long *v, size_t n) {
-    const size_t nb = (n + 1023) / 1024;
-    if (sums.n < nb) sums.alloc(nb);
-    unsigned long long *sp = sums.p;
-    k_flt_scan1<<<(unsigned)nb, 256, 0, s>>>(v, sp, n);
-    k_flt_scan2<<<1, 1024, 0, s>>>(sp, nb);
-    k_flt_scan3<<<(unsigned)nb, 256, 0, s>>>(v, sp, n);
-    launches += 3;
-  }
-};
-
-bool is_acgt(const std::string &s) {
-  for (char c : s) if (c != 'A' && c != 'C' && c != 'G' && c != 'T') return false;
-  return true;
+void dd2::flt_check_reads(const char *seq, const uint8_t *qual, long long nbytes, unsigned *err, cudaStream_t s) {
+  k_flt_alpha<<<(unsigned)((nbytes + 255) / 256), 256, 0, s>>>(seq, qual, nbytes, err);
 }
+
+void dd2::FltScan::operator()(unsigned long long *v, size_t n) {
+  const size_t nb = (n + 1023) / 1024;
+  if (sums.n < nb) sums.alloc(nb);
+  unsigned long long *sp = sums.p;
+  k_flt_scan1<<<(unsigned)nb, 256, 0, s>>>(v, sp, n);
+  k_flt_scan2<<<1, 1024, 0, s>>>(sp, nb);
+  k_flt_scan3<<<(unsigned)nb, 256, 0, s>>>(v, sp, n);
+  launches += 3;
+}
+
+namespace {
 
 // The word-mers of the circularised ref (ref + ref[0:w], C_matchRef's phash) and, with both, of its reverse complement
 // (isPhiX's rc.phix), as the device's hash table: strand mask 1 = ref, 2 = reverse complement.
@@ -495,26 +473,6 @@ std::vector<unsigned long long> build_table(const std::string &ref, int w, bool 
     }
   }
   return t;
-}
-
-void need_device(int32_t device) {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) throw BErr{"dada2b: no CUDA device available (this library has no CPU path)."};
-  BCK(cudaSetDevice(device));
-}
-
-// Offsets relative to the first read; returns the bytes spanned.
-long long rebase(int n, const int64_t *seq_off, std::vector<long long> &off) {
-  off.resize((size_t)n + 1);
-  const long long o0 = seq_off[0];
-  for (int r = 0; r < n; r++) {
-    const long long l = seq_off[r + 1] - seq_off[r];
-    if (l < 0) throw BErr{"Bad sequence offsets."};
-    if (l > INT_MAX / 2) throw BErr{"dada2b: read too long."};
-    off[r] = seq_off[r] - o0;
-  }
-  off[n] = seq_off[n] - o0;
-  return off[n];
 }
 
 FltMateOpt mate_opt(const dada2b_filter_mate_opts &m, bool paired) {
@@ -632,7 +590,7 @@ int run_filter(const dada2b_derep_in *fwd, const dada2b_derep_in *rev, const dad
     for (int m = 0; m < nm; m++) {
       if (nbytes[m]) {
         const char *sp = d_seq[m].p; const uint8_t *qp = d_qual[m].p; unsigned *ep = d_err.p; const long long nb = nbytes[m];
-        k_flt_alpha<<<(unsigned)((nb + 255) / 256), 256, 0, s>>>(sp, qp, nb, ep);
+        flt_check_reads(sp, qp, nb, ep, s);
         launches++; kbytes += 2 * nb;
       }
     }

@@ -2,6 +2,7 @@
 
     accumulateTrans   /root/reference/R/errorModels.R:462-471
     loessErrfun       /root/reference/R/errorModels.R:28-67
+    PacBioErrfun      R/errorModels.R:183-196 (reference)
     dada(selfConsist=TRUE) / learnErrors loop   /root/reference/R/dada.R:256-391, R/errorModels.R:270-330
 
 The reference does these steps in R between the <= 11 dada_uniques() passes; they see a 16 x Q matrix, so they stay on the
@@ -110,6 +111,22 @@ def loessErrfun(trans, span=0.75, degree=2):
                      est[6:8], 1 - est[6:9].sum(axis=0), est[8],
                      est[9:12], 1 - est[9:12].sum(axis=0)])
     return err
+
+
+def PacBioErrfun(trans):
+    """16 x Q transition counts -> 16 x Q error rates for reads whose qualities reach 93 (R/errorModels.R:183-196).
+    Column j is quality score j, so R's `"93" %in% colnames(trans)` is Q >= 94.  Columns 0..92 are loessErrfun's fit;
+    column 93 is the observed rate with pseudo-counts, (count + 1) / (total of the source base + 4)."""
+    trans = np.asarray(trans, dtype=np.float64)
+    Q = trans.shape[1]
+    if Q < 94:
+        print("The max qual score of 93 was not detected. Using standard error fitting.")
+        return loessErrfun(trans)
+    if Q > 94:
+        raise ValueError("Max qual score of 93 not the last column as expected.")
+    err = loessErrfun(trans[:, :93])
+    tot93 = np.repeat(trans[:, 93].reshape(4, 4).sum(axis=1), 4)
+    return np.hstack([err, ((trans[:, 93] + 1.0) / (tot93 + 4.0))[:, None]])
 
 
 def getErrors_enforce(err):
