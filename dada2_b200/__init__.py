@@ -12,3 +12,6 @@ from .filter import filterAndTrim, filter_reads  # noqa: F401,E402
 from . import primer  # noqa: F401,E402
 from .primer import removePrimers, remove_primers_reads  # noqa: F401,E402
 from .errmodel import PacBioErrfun  # noqa: F401,E402
+from .derep import pool_dereps  # noqa: F401,E402
+from . import denoise  # noqa: F401,E402
+from .denoise import dada, learnErrors  # noqa: F401,E402

@@ -20,6 +20,7 @@
 #include "dd_bimera.cuh"
 #include "dd_hostutil.h"
 #include "dd_ctx.h"
+#include "dd_sort.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -27,12 +28,6 @@
 #include <cstring>
 
 namespace dd2 {
-
-constexpr int RS_TILE = 2048;          // elements per (one-warp) block of a radix pass
-
-// digit of element `id` in this pass: byte `shift/8` of keys[id * stride + word]
-struct RsPass { const uint32_t *keys; int stride, word, shift; };
-__device__ __forceinline__ unsigned rs_digit(const RsPass &p, uint32_t id) { return (p.keys[(size_t)id * p.stride + p.word] >> p.shift) & 255u; }
 
 __global__ void __launch_bounds__(32) k_rs_hist(RsPass p, const uint32_t *src, unsigned n, uint32_t *hist, unsigned nb) {
   __shared__ uint32_t h[256];
@@ -139,12 +134,6 @@ __global__ void __launch_bounds__(256) k_scan3(uint32_t *out, const uint32_t *su
 }
 
 // ---- dereplication kernels ----
-struct DrIn {
-  int nreads, KW, maxlen;              // KW = key words per read
-  const char *seq; const uint8_t *qual; const long long *off;
-  uint32_t *keys;                      // [nreads][KW + 1]: MSB-first packed bases, then the length
-  unsigned long long *flags;           // [0] bad base seen
-};
 __global__ void __launch_bounds__(256) k_dr_pack(DrIn a) {
   const size_t x = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int S = a.KW + 1;
@@ -254,12 +243,7 @@ __global__ void __launch_bounds__(256) k_dr_map(const uint32_t *head, const uint
   map[id] = (int32_t)rank_of[seg[p] + head[p] - 1] + 1;
 }
 
-// dereplication -> dada(): fill a context's packed arrays from the device-side result (one thread per 16-base word / per quality byte)
-struct DrToCtx {
-  DevIn in; unsigned nuniq; int maxlen, S;
-  const char *seq; const long long *off; const int32_t *rep, *abund; const double *quals; const uint32_t *keys;
-  unsigned long long *maxq;
-};
+// dereplication / pooling -> dada(): fill a context's packed arrays from the device-side result
 __global__ void __launch_bounds__(256) k_dr_to_ctx(DrToCtx a) {
   const size_t x = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t per = (size_t)a.in.SW + a.in.QS;
@@ -275,7 +259,7 @@ __global__ void __launch_bounds__(256) k_dr_to_ctx(DrToCtx a) {
       if (p < len) { const char c = a.seq[o + p]; v |= (uint32_t)(c == 'C' ? 1 : (c == 'G' ? 2 : (c == 'T' ? 3 : 0))) << (2 * b); }
     }
     a.in.seq2[(size_t)r * a.in.SW + w] = v;
-    if (w == 0) { a.in.len[r] = (uint16_t)len; a.in.reads[r] = (uint32_t)a.abund[r]; a.in.prior[r] = 0; }
+    if (w == 0) { a.in.len[r] = (uint16_t)len; a.in.reads[r] = (uint32_t)a.abund[r]; a.in.prior[r] = a.prior ? a.prior[r] : 0; }
   } else {                                               // (uint8_t) round(mean quality), containers.cpp:34 (same rounding as do_upload)
     const int p = w - a.in.SW;
     uint8_t q = 0;
@@ -290,41 +274,32 @@ __global__ void __launch_bounds__(256) k_dr_to_ctx(DrToCtx a) {
   }
 }
 
+
+void Sorter::scan(uint32_t *buf, size_t n) {
+  const size_t nb = (n + 1023) / 1024;
+  if (sums.n < nb) sums.alloc(nb);
+  uint32_t *sp = sums.p;
+  k_scan1<<<(unsigned)nb, 256, 0, s>>>(buf, buf, sp, n);
+  k_scan2<<<1, 1024, 0, s>>>(sp, nb);
+  k_scan3<<<(unsigned)nb, 256, 0, s>>>(buf, sp, n);
+  launches += 3;
+}
+void Sorter::pass(const RsPass &p, const uint32_t *a, uint32_t *b, unsigned n) {
+  const unsigned nb = (n + RS_TILE - 1) / RS_TILE;
+  if (hist.n < (size_t)256 * nb) hist.alloc((size_t)256 * nb);
+  if (!total.p) total.alloc(1);
+  uint32_t *hp = hist.p, *tp = total.p;
+  k_rs_hist<<<nb, 32, 0, s>>>(p, a, n, hp, nb);
+  k_rs_total<<<1, 256, 0, s>>>(hp, nb, tp);
+  launches += 2;
+  scan(hp, (size_t)256 * nb);
+  k_rs_scatter<<<nb, 32, 0, s>>>(p, a, b, n, hp, nb, tp);
+  launches += 1;
+}
+
 }  // namespace dd2
 
 using namespace dd2;
-
-namespace {
-
-struct Sorter {                       // stable LSD radix sort of an index array by byte digits
-  cudaStream_t s;
-  BBuf<uint32_t> hist, sums, total;
-  long long launches = 0;
-  void scan(uint32_t *buf, size_t n) {
-    const size_t nb = (n + 1023) / 1024;
-    if (sums.n < nb) sums.alloc(nb);
-    uint32_t *sp = sums.p;
-    k_scan1<<<(unsigned)nb, 256, 0, s>>>(buf, buf, sp, n);
-    k_scan2<<<1, 1024, 0, s>>>(sp, nb);
-    k_scan3<<<(unsigned)nb, 256, 0, s>>>(buf, sp, n);
-    launches += 3;
-  }
-  // sorts a[0..n) by digit `pass`; result in b; caller swaps
-  void pass(const RsPass &p, const uint32_t *a, uint32_t *b, unsigned n) {
-    const unsigned nb = (n + RS_TILE - 1) / RS_TILE;
-    if (hist.n < (size_t)256 * nb) hist.alloc((size_t)256 * nb);
-    if (!total.p) total.alloc(1);
-    uint32_t *hp = hist.p, *tp = total.p;
-    k_rs_hist<<<nb, 32, 0, s>>>(p, a, n, hp, nb);
-    k_rs_total<<<1, 256, 0, s>>>(hp, nb, tp);
-    launches += 2;
-    scan(hp, (size_t)256 * nb);
-    k_rs_scatter<<<nb, 32, 0, s>>>(p, a, b, n, hp, nb, tp);
-    launches += 1;
-  }
-};
-
-}  // namespace
 
 extern "C" {
 

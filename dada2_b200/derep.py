@@ -26,6 +26,21 @@ class DerepOut(C.Structure):
                 ("ms_device", C.c_double), ("ms_sort", C.c_double), ("ms_total", C.c_double)]
 
 
+class PoolIn(C.Structure):
+    _fields_ = [("nsamples", C.c_int32), ("nuniq", C.c_void_p), ("maxlen", C.c_void_p), ("nmap", C.c_void_p), ("seq_concat", C.c_char_p),
+                ("seq_off", C.c_void_p), ("abund", C.c_void_p), ("quals", C.c_void_p), ("map", C.c_void_p), ("prior", C.c_void_p)]
+
+
+class PoolOut(C.Structure):
+    _fields_ = [("npool", C.c_int32), ("maxlen", C.c_int32), ("nuniq_in", C.c_int64), ("nmap", C.c_int64),
+                ("seq_concat", C.POINTER(C.c_char)), ("seq_off", C.POINTER(C.c_int64)), ("abund", C.POINTER(C.c_int32)),
+                ("quals", C.POINTER(C.c_double)), ("map", C.POINTER(C.c_int32)), ("index", C.POINTER(C.c_int32)),
+                ("prior", C.POINTER(C.c_uint8)), ("qmax", C.c_double), ("gpu_launches", C.c_int64), ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64),
+                ("ms_h2d", C.c_double), ("ms_kernels", C.c_double), ("ms_d2h", C.c_double), ("ms_total", C.c_double)]
+
+
+POOL_STATS = ("gpu_launches", "h2d_bytes", "d2h_bytes", "ms_h2d", "ms_kernels", "ms_d2h", "ms_total")
+
 _BOUND = False
 
 
@@ -37,6 +52,9 @@ def _lib():
         L.dada2b_derep.argtypes = [P(DerepIn), C.c_int32, P(P(DerepOut)), C.c_char_p]
         L.dada2b_derep_free.argtypes = [P(DerepOut)]
         L.dada2b_derep_resident.argtypes = [P(DerepIn), C.c_int32, C.c_int32, P(P(DerepOut)), P(C.c_void_p), C.c_char_p]
+        L.dada2b_pool.argtypes = [P(PoolIn), C.c_int32, C.c_int32, P(P(PoolOut)), C.c_char_p]
+        L.dada2b_pool_resident.argtypes = [P(PoolIn), C.c_int32, C.c_int32, P(P(PoolOut)), P(C.c_void_p), C.c_char_p]
+        L.dada2b_pool_free.argtypes = [P(PoolOut)]
         _BOUND = True
     return L
 
@@ -154,3 +172,72 @@ def combineDereps2(dereps):
     newmap = rank[np.concatenate(maps) - 1] + 1 if maps else np.zeros(0, np.int64)
     return {"uniques": [seqs[i] for i in order], "abundances": counts[order].astype(np.int32), "quals": quals[order],
             "map": newmap.astype(np.int32)}
+
+
+def pool_dereps(dereps, want_quals=True, device=0, priors=None, resident=False, return_stats=False):
+    """combineDereps2 (R/multiSample.R:165-203) on the device (include/dada2b_pool.h): a list of derep dicts -> one derep
+    dict (uniques, abundances, quals [npool, maxlen] or None without want_quals, map) equal to combineDereps2's, plus
+    `index` (int32 per sample-unique, concatenated sample by sample: 1-based pooled position, match(names(derep_s$uniques),
+    names(pooled))), `qmax` (largest non-NA pooled mean) and `prior` (bool per pooled unique: OR of `priors`, one bool array per sample, over the occurrences).
+    resident=True: additionally leaves the pooled uniques packed on the device with their prior flags and returns
+    (dict, dada2_b200.Resident); run(err) on it is dada() on the pooled derep."""
+    if isinstance(dereps, dict):
+        dereps = [dereps]
+    L = _lib()
+    S = len(dereps)
+    seqs = [u for d in dereps for u in d["uniques"]]
+    nuniq = np.array([len(d["uniques"]) for d in dereps], np.int32)
+    qs = [np.asarray(d["quals"], dtype=np.float64) for d in dereps]
+    for d, q in zip(dereps, qs):
+        if q.ndim != 2 or q.shape[0] != len(d["uniques"]):
+            raise api.Dada2bError("derep$quals matrices must have one row for each derep$unique sequence.")
+    maxlen = np.array([q.shape[1] for q in qs], np.int32)
+    maps = [np.asarray(d["map"], dtype=np.int32).ravel() for d in dereps]
+    nmap = np.array([len(m) for m in maps], np.int64)
+    lens = np.fromiter((len(x) for x in seqs), dtype=np.int64, count=len(seqs))
+    off = np.zeros(len(seqs) + 1, np.int64)
+    np.cumsum(lens, out=off[1:])
+    buf = "".join(seqs).encode()
+    ab = np.ascontiguousarray(np.concatenate([np.asarray(d["abundances"]) for d in dereps]) if S else np.zeros(0), dtype=np.int32)
+    if len(ab) != len(seqs):
+        raise api.Dada2bError("derep$uniques and its abundances have different lengths.")
+    qcat = np.ascontiguousarray(np.concatenate([q.ravel() for q in qs]) if S else np.zeros(0))
+    mcat = np.ascontiguousarray(np.concatenate(maps) if S else np.zeros(0, np.int32))
+    pr = None
+    if priors is not None:
+        pr = np.ascontiguousarray(np.concatenate([np.asarray(p, dtype=bool).ravel() for p in priors]), dtype=np.uint8)
+        if len(pr) != len(seqs):
+            raise api.Dada2bError("Sequence and priors vectors had different lengths.")
+    inp = PoolIn(S, nuniq.ctypes.data, maxlen.ctypes.data, nmap.ctypes.data, buf, off.ctypes.data, ab.ctypes.data, qcat.ctypes.data,
+                 mcat.ctypes.data, pr.ctypes.data if pr is not None else None)
+    out = C.POINTER(PoolOut)()
+    eb = C.create_string_buffer(ERRLEN)
+    ctx = C.c_void_p()
+    if resident:
+        rc = L.dada2b_pool_resident(C.byref(inp), int(device), int(bool(want_quals)), C.byref(out), C.byref(ctx), eb)
+    else:
+        rc = L.dada2b_pool(C.byref(inp), int(device), int(bool(want_quals)), C.byref(out), eb)
+    if rc:
+        raise api.Dada2bError(eb.value.decode())
+    try:
+        r = out.contents
+        nu, ml = r.npool, r.maxlen
+        so = np.ctypeslib.as_array(r.seq_off, shape=(nu + 1,)).copy()
+        raw = C.string_at(r.seq_concat, int(so[-1])).decode()
+        res = {"uniques": [raw[so[i]:so[i + 1]] for i in range(nu)],
+               "abundances": np.ctypeslib.as_array(r.abund, shape=(nu,)).copy(),
+               "quals": np.ctypeslib.as_array(r.quals, shape=(nu, ml)).copy() if r.quals else None,
+               "map": np.ctypeslib.as_array(r.map, shape=(max(r.nmap, 1),))[:r.nmap].copy(),
+               "index": np.ctypeslib.as_array(r.index, shape=(r.nuniq_in,)).copy(),
+               "prior": np.ctypeslib.as_array(r.prior, shape=(nu,)).astype(bool), "qmax": r.qmax}
+        if return_stats:
+            res["stats"] = {k: getattr(r, k) for k in POOL_STATS}
+        if resident:
+            rs = api.Resident.__new__(api.Resident)                 # adopt the context the library built on the device
+            rs._pin = None
+            rs._ctx = ctx
+            rs.nraw = nu
+            return res, rs
+        return res
+    finally:
+        L.dada2b_pool_free(out)

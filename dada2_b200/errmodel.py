@@ -3,7 +3,8 @@
     accumulateTrans   /root/reference/R/errorModels.R:462-471
     loessErrfun       /root/reference/R/errorModels.R:28-67
     PacBioErrfun      R/errorModels.R:183-196 (reference)
-    dada(selfConsist=TRUE) / learnErrors loop   /root/reference/R/dada.R:256-391, R/errorModels.R:270-330
+    dada(selfConsist=TRUE) / learnErrors loop   /root/reference/R/dada.R:256-391, R/errorModels.R:270-330 (consist_loop;
+                                                dada_selfconsist / learnErrors below run it on one resident sample)
 
 The reference does these steps in R between the <= 11 dada_uniques() passes; they see a 16 x Q matrix, so they stay on the
 host here as well (R is not in this image: Python mirrors the R functions name for name, like dada2_b200/api.py does for
@@ -141,13 +142,14 @@ def getErrors_enforce(err):
     return err
 
 
-def dada_selfconsist(runner, ncol=41, err=None, errorEstimationFunction=loessErrfun, MAX_CONSIST=10, selfConsist=True, verbose=False,
-                     on_pass=None):
-    """The main loop of dada() (R/dada.R:256-391) for one (pooled) sample whose uniques are resident on the device.
+def consist_loop(runners, err=None, errorEstimationFunction=loessErrfun, MAX_CONSIST=10, selfConsist=True, verbose=False,
+                 pseudo=None, on_pass=None):
+    """The main loop of dada() (R/dada.R:256-391) over samples.
 
-    runner(err, max_clust) -> result dict of one dada_uniques() pass (e.g. `lambda e, mc: resident.run(e, max_clust=mc)`).
-    err = None: learnErrors' start (initializeErr: all-ones matrix, MAX_CLUST = 1, R/dada.R:297-299, :342).
-    Returns (last result, final err, list of the err matrices tried, number of passes)."""
+    runners[i](err, max_clust) -> the dada_uniques() result of sample i.  err = None: the loop starts from initializeErr
+    (R/dada.R:297-299, :342): every runner is called with err None and max_clust 1 and builds its own all-ones matrix.
+    pseudo(results) is called where R computes the pseudo priors of pool = "pseudo" (:380-384); the loop then always runs
+    a second pass.  Returns (results of the last pass, final err, list of the err matrices tried, number of passes)."""
     initializeErr = err is None
     nconsist = 0 if initializeErr else 1
     errs = []
@@ -155,12 +157,11 @@ def dada_selfconsist(runner, ncol=41, err=None, errorEstimationFunction=loessErr
     while True:
         if nconsist > 0:
             errs.append(err)
-        erri = np.ones((16, ncol)) if initializeErr else np.asarray(err, dtype=np.float64)
-        res = runner(erri, 1 if initializeErr else 0)
+        results = [run(None if initializeErr else err, 1 if initializeErr else 0) for run in runners]
         npass += 1
         if on_pass:
-            on_pass(npass, nconsist, res)
-        cur = accumulateTrans([res["subqual"]])
+            on_pass(npass, nconsist, results)
+        cur = accumulateTrans([r["subqual"] for r in results])
         try:
             err = errorEstimationFunction(cur) if errorEstimationFunction is not None else None
         except ValueError:
@@ -174,9 +175,27 @@ def dada_selfconsist(runner, ncol=41, err=None, errorEstimationFunction=loessErr
             err = np.array(err, dtype=np.float64)
             err[[0, 5, 10, 15], :] = 1.0                      # self-transitions of the initial estimate forced to 1 (R/dada.R:385-388)
         if (not selfConsist) or any(e is not None and err is not None and np.array_equal(e, err) for e in errs) or nconsist >= MAX_CONSIST:
-            break
+            if pseudo is None or nconsist >= 2:
+                break
+        if pseudo is not None and nconsist >= 1:
+            pseudo(results)
         nconsist += 1
-    return res, err, errs, npass
+    return results, err, errs, npass
+
+
+def dada_selfconsist(runner, ncol=41, err=None, errorEstimationFunction=loessErrfun, MAX_CONSIST=10, selfConsist=True, verbose=False,
+                     on_pass=None):
+    """consist_loop for one (pooled) sample whose uniques are resident on the device.
+
+    runner(err, max_clust) -> result dict of one dada_uniques() pass (e.g. `lambda e, mc: resident.run(e, max_clust=mc)`).
+    err = None: learnErrors' start (initializeErr: all-ones 16 x ncol matrix, MAX_CLUST = 1).
+    Returns (last result, final err, list of the err matrices tried, number of passes)."""
+    def one(e, mc):
+        return runner(np.ones((16, ncol)) if e is None else np.asarray(e, dtype=np.float64), mc)
+    hook = (lambda n, c, rs: on_pass(n, c, rs[0])) if on_pass else None
+    results, err, errs, npass = consist_loop([one], err=err, errorEstimationFunction=errorEstimationFunction, MAX_CONSIST=MAX_CONSIST,
+                                             selfConsist=selfConsist, verbose=verbose, on_pass=hook)
+    return results[0], err, errs, npass
 
 
 def learnErrors(runner, ncol=41, errorEstimationFunction=loessErrfun, MAX_CONSIST=10, verbose=False, on_pass=None):
