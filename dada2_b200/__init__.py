@@ -15,3 +15,5 @@ from .errmodel import PacBioErrfun  # noqa: F401,E402
 from .derep import pool_dereps  # noqa: F401,E402
 from . import denoise  # noqa: F401,E402
 from .denoise import dada, learnErrors  # noqa: F401,E402
+from . import taxonomy  # noqa: F401,E402
+from .taxonomy import TaxDB, assignTaxonomy  # noqa: F401,E402
