@@ -48,6 +48,11 @@ def lib():
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p]
         L.dada2b_test_screen.argtypes = [C.c_void_p, C.c_uint32, P(_abi.Opts), C.c_double, C.c_uint32, C.c_void_p, C.c_int32, C.c_int32,
                                          C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p]
+        L.dada2b_test_raw_bounds.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                             C.c_char_p]
+        L.dada2b_test_bound.argtypes = [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_int32, P(_abi.Opts), C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_char_p]
         _LIB = L
     return _LIB
 
@@ -188,6 +193,43 @@ class Resident:
         if rc:
             raise Dada2bError(eb.value.decode())
         return dict(kind=kind, minsum=minsum, counters=dict(zip(("align", "shroud", "gapless", "nw"), ctr.tolist())))
+
+    def test_raw_bounds(self, err, use_quals=True, rank=0, world=1):
+        """Kernel-level hook (include/dada2b_test.h): k_raw_bounds' per-raw factors (S, rho) of the two-phase bound for the raws
+        of shard (rank, world); NaN for the other raws."""
+        e = _check_err(err)
+        ecm = np.asfortranarray(e)
+        S = np.zeros(self.nraw, np.float64); rho = np.zeros(self.nraw, np.float64)
+        eb = C.create_string_buffer(_abi.ERRLEN)
+        rc = lib().dada2b_test_raw_bounds(self._ctx, ecm.ctypes.data, int(e.shape[1]), int(bool(use_quals)), int(rank), int(world),
+                                          S.ctypes.data, rho.ctypes.data, eb)
+        if rc:
+            raise Dada2bError(eb.value.decode())
+        return S, rho
+
+    def test_bound(self, which, centre, cluster_i, jobs, e_minmax, err, njobs_hint=0, **opts):
+        """Kernel-level hook (include/dada2b_test.h): one launch of a bound-testing loop kernel (0 k_nwrow<BOUND>, 1 k_nwlane,
+        2 k_nwfwd's bound pass, 3 k_gapless_loop) over the job list -> outcome per job (0 dropped, 1 survivor list, 2 gapless
+        list, 3 handed back, 4 stored, 5 passed the bound, not stored), nsubs, lambda (stored lambda, NaN otherwise), e_after
+        (E_minmax after the launch) and counters {surv, gapless, back, stored}."""
+        e = _check_err(err)
+        ecm = np.asfortranarray(e)
+        o = _abi.make_opts(**_normalise_opts(dict(opts)))
+        jobs = np.ascontiguousarray(jobs, dtype=np.uint32)
+        em = np.ascontiguousarray(e_minmax, dtype=np.float64)
+        if len(em) != self.nraw:
+            raise ValueError("e_minmax needs one entry per raw")
+        n = len(jobs)
+        outcome = np.zeros(n, np.int32); nsubs = np.zeros(n, np.int32); lam = np.zeros(n, np.float64)
+        e_after = np.zeros(self.nraw, np.float64); ctr = np.zeros(4, np.int64)
+        eb = C.create_string_buffer(_abi.ERRLEN)
+        rc = lib().dada2b_test_bound(self._ctx, int(which), int(centre), int(cluster_i), n, jobs.ctypes.data, em.ctypes.data, ecm.ctypes.data,
+                                     int(e.shape[1]), C.byref(o), int(njobs_hint), outcome.ctypes.data, nsubs.ctypes.data, lam.ctypes.data,
+                                     e_after.ctypes.data, ctr.ctypes.data, eb)
+        if rc:
+            raise Dada2bError(eb.value.decode())
+        return dict(outcome=outcome, nsubs=nsubs, lam=lam, e_after=e_after,
+                    counters=dict(zip(("surv", "gapless", "back", "stored"), ctr.tolist())))
 
     def close(self):
         if getattr(self, "_ctx", None) and self._ctx.value:

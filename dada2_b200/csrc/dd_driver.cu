@@ -23,6 +23,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 #include <string>
 #if defined(__SSE2__)
 #include <emmintrin.h>
@@ -1815,6 +1816,148 @@ static void do_test_loop_nw(dada2b_ctx *cx, int which, int npairs, const uint32_
   }
 }
 
+// Per-raw factors of the two-phase bound (include/dada2b_test.h): k_raw_bounds over the raws of shard (rank, world), launched as
+// do_run launches it; the other raws keep NaN.
+static void do_test_raw_bounds(dada2b_ctx *cx, const double *err_cm, int Q, int use_quals, int rank, int world, double *S, double *rho) {
+  CK(cudaSetDevice(cx->device));
+  if (Q < 1) throw Err{"Error matrix must have 16 rows."};
+  if (world < 1 || rank < 0 || rank >= world) throw Err{"dada2b_test_raw_bounds: bad rank/world"};
+  if (use_quals && cx->maxq > Q - 1) throw Err{"Rounded quality exceeded range of err lookup table."};
+  const size_t n = (size_t)cx->in.nraw;
+  std::vector<double> e((size_t)16 * Q);
+  for (int r = 0; r < 16; r++) for (int c = 0; c < Q; c++) e[(size_t)r * Q + c] = err_cm[r + 16 * (size_t)c];
+  DBuf<double> d_err, d_S, d_rho;
+  d_err.alloc(e.size()); d_S.alloc(n); d_rho.alloc(n);
+  CK(cudaMemcpyAsync(d_err.p, e.data(), e.size() * 8, cudaMemcpyHostToDevice, cx->stream));
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  launch_fill_f64(d_S.p, nan, n, cx->stream); launch_fill_f64(d_rho.p, nan, n, cx->stream);
+  launch_raw_bounds(cx->in, d_err.p, Q, use_quals != 0, d_S.p, d_rho.p, rank, world, cx->stream);
+  CK(cudaMemcpyAsync(S, d_S.p, n * 8, cudaMemcpyDeviceToHost, cx->stream));
+  CK(cudaMemcpyAsync(rho, d_rho.p, n * 8, cudaMemcpyDeviceToHost, cx->stream));
+  CK(cudaStreamSynchronize(cx->stream));
+}
+
+// The bound pass of one round (include/dada2b_test.h): ONE launch of one bound-testing loop kernel over the caller's job list, with
+// the caller's E_minmax per raw and cluster index, as Run::launch_compare launches it.  Every list the kernel writes is read back and
+// checked: each raw at most once over all lists, only jobs, counts within the job count.
+static void do_test_bound(dada2b_ctx *cx, int which, uint32_t centre, uint32_t cluster_i, int64_t njobs, const uint32_t *jobs, const double *e_minmax,
+                          const double *err_cm, int Q, const dada2b_opts *o, uint64_t njobs_hint, int32_t *outcome, int32_t *nsubs, double *lambda,
+                          double *e_after, int64_t *counters) {
+  CK(cudaSetDevice(cx->device));
+  if (cx->bad_nt) throw Err{"Unexpected nucleotide."};
+  if (Q < 1) throw Err{"Error matrix must have 16 rows."};
+  if (o->use_quals && cx->maxq > Q - 1) throw Err{"Rounded quality exceeded range of err lookup table."};
+  if (which < 0 || which > 3) throw Err{"dada2b_test_bound: which must be 0 (k_nwrow<BOUND>), 1 (k_nwlane), 2 (k_nwfwd) or 3 (k_gapless_loop)"};
+  if (cluster_i < 1) throw Err{"dada2b_test_bound: cluster_i must be >= 1 (cluster 0 never tests the bound)"};
+  const size_t n = (size_t)cx->in.nraw;
+  if (centre >= n) throw Err{"dada2b_test_bound: centre out of range"};
+  if (njobs < 1 || (size_t)njobs > n) throw Err{"dada2b_test_bound: njobs must be in 1 .. nraw"};
+  std::vector<int64_t> job_of(n, -1);
+  for (int64_t k = 0; k < njobs; k++) {
+    if (jobs[k] >= n) throw Err{"dada2b_test_bound: job out of range"};
+    if (job_of[jobs[k]] >= 0) throw Err{"dada2b_test_bound: a raw appears twice in the job list"};
+    job_of[jobs[k]] = k;
+  }
+  Run R;
+  R.bind(cx, o, Q);
+  R.setup_params();
+  R.alloc_state();
+  if (!R.two_phase) throw Err{"dada2b_test_bound: homopolymer gap costs have no bound pass"};
+  cudaStream_t s = R.s;
+  {
+    std::vector<double> e((size_t)16 * Q);
+    for (int r = 0; r < 16; r++) for (int c = 0; c < Q; c++) e[(size_t)r * Q + c] = err_cm[r + 16 * (size_t)c];
+    R.h2d(R.err.p, e.data(), e.size() * 8);
+  }
+  launch_raw_bounds(R.in, R.err.p, Q, o->use_quals != 0, R.raw_S.p, R.raw_rho.p, cx->rank, cx->world, s);
+  R.h2d(R.E_minmax.p, e_minmax, n * 8);
+  R.ensure_cs_cap(n + (unsigned long long)njobs + 1024);    // cluster 0 owns entries [0, nraw); a later cluster takes slots by atomics
+  const uint64_t nj = (uint64_t)njobs;
+  DBuf<uint32_t> d_jobs, l_back, l_surv, l_gl, d_ns; DBuf<unsigned long long> cnt;
+  d_jobs.alloc(nj); l_back.alloc(nj + 2); l_surv.alloc(nj); l_gl.alloc(nj); d_ns.alloc(n); cnt.alloc(4);
+  R.h2d(d_jobs.p, jobs, nj * 4);
+  cnt.zero(s);
+  R.h2d(cnt.p, &nj, 8);                               // cnt[0] = job count, [1] handed back, [2] survivors, [3] gapless-listed
+  CK(cudaMemsetAsync(d_ns.p, 0xFF, n * 4, s));
+  FwdArgs f{};
+  f.in = R.in; f.P = R.P; f.st = R.st; f.jobs = d_jobs.p; f.njobs_ptr = cnt.p;
+  f.centre_idx = centre; f.centre_reads = cx->reads[centre]; f.cluster_i = cluster_i; f.total_reads = cx->total_reads;
+  f.fb_list = l_back.p; f.fb_count = cnt.p + 1; f.seq_bytes = R.seq_bytes; f.mode = 0; f.job_mul = 1; f.job_add = 0;
+  {
+    const long worst = (long)R.in.maxlen * std::max(std::abs(R.P.mismatch), std::abs(R.P.match)) + std::max(std::abs(R.P.gap), std::abs(R.P.hgap)) + 16;
+    f.fast_ok = (worst < std::abs((long)R.P.sentinel) / 2) ? 1 : 0;
+  }
+  f.raw_S = R.raw_S.p; f.raw_rho = R.raw_rho.p; f.surv_list = l_surv.p; f.surv_count = cnt.p + 2;
+  const int len1 = (int)cx->len[centre];
+  bool launched = false;
+  if (which == 0) {
+    f.gl_out = l_gl.p; f.gl_count = cnt.p + 3;
+    launched = launch_nwrow_bound(f, l_back.p, cnt.p + 1, len1, nj, cx->num_sms, 0ull, s, d_ns.p);
+  } else if (which == 1) {
+    if (!R.lane_max || !R.lane_mv.p) throw Err{"dada2b_test_bound: k_nwlane is not set up for this configuration"};
+    if (nj > R.lane_max) throw Err{"dada2b_test_bound: more jobs than k_nwlane takes (lane_max)"};
+    f.ns_out = d_ns.p;
+    launched = launch_nwlane(f, l_back.p, cnt.p + 1, R.lane_mv.p, R.lane_sub.p, len1, R.lane_max, (int)R.lane_max, s);
+  } else if (which == 2) {
+    if (R.P.band < 0) throw Err{"dada2b_test_bound: k_nwfwd needs a band"};
+    f.ns_out = d_ns.p;
+    launched = launch_nwfwd(f, R.fwd_slots, nj, njobs_hint, cx->num_sms, s, true);
+  } else {
+    f.ns_out = d_ns.p;
+    launch_gapless_loop(f, 1, nj, cx->num_sms, s);
+    launched = true;
+  }
+  if (!launched) throw Err{"dada2b_test_bound: the kernel does not take this configuration"};
+  unsigned long long hc[4];
+  std::vector<double> E2(n);
+  std::vector<uint32_t> ns(n);
+  R.d2h(hc, cnt.p, 32); R.d2h(E2.data(), R.E_minmax.p, n * 8); R.d2h(ns.data(), d_ns.p, n * 4);
+  R.read_ctr();
+  R.check_dev_error();
+  const unsigned long long nstored = R.h_ctr.p[CTR_CS_COUNT] - n;
+  if (hc[0] != nj || hc[1] > nj || hc[2] > nj || hc[3] > nj || nstored > nj || hc[1] + hc[2] + hc[3] > nj)
+    throw Err{"dada2b_test_bound: a list count is out of range"};
+  std::vector<uint32_t> back(hc[1]), surv(hc[2]), gl(hc[3]), cs_idx(nstored), cs_ham(nstored), cs_i(nstored);
+  std::vector<double> cs_lam(nstored);
+  R.d2h(back.data(), l_back.p, hc[1] * 4); R.d2h(surv.data(), l_surv.p, hc[2] * 4); R.d2h(gl.data(), l_gl.p, hc[3] * 4);
+  R.d2h(cs_idx.data(), R.st.cs_index + n, nstored * 4); R.d2h(cs_ham.data(), R.st.cs_ham + n, nstored * 4);
+  R.d2h(cs_i.data(), R.st.cs_i + n, nstored * 4); R.d2h(cs_lam.data(), R.st.cs_lambda + n, nstored * 8);
+  R.sync();
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  for (int64_t k = 0; k < njobs; k++) { outcome[k] = -1; nsubs[k] = -1; lambda[k] = nan; }
+  auto mark = [&](uint32_t r, int32_t v, const char *what) {
+    if (r >= n || job_of[r] < 0) throw Err{std::string("dada2b_test_bound: a raw that is no job appears in the ") + what};
+    if (outcome[job_of[r]] >= 0) throw Err{std::string("dada2b_test_bound: a raw appears twice in the lists (") + what + ")"};
+    outcome[job_of[r]] = v;
+  };
+  for (uint32_t r : surv) mark(r, 1, "survivor list");
+  for (uint32_t r : gl) mark(r, 2, "gapless list");
+  for (uint32_t r : back) mark(r, 3, "hand-back list");
+  for (size_t k = 0; k < nstored; k++) {
+    if (cs_i[k] != cluster_i) throw Err{"dada2b_test_bound: a stored comparison carries another cluster index"};
+    mark(cs_idx[k], 4, "comparison store");
+    lambda[job_of[cs_idx[k]]] = cs_lam[k];
+    if (cs_ham[k] != (ns[cs_idx[k]] & 0x7FFFFFFFu)) throw Err{"dada2b_test_bound: the stored hamming differs from the bound pass's nsubs"};
+  }
+  for (int64_t k = 0; k < njobs; k++) {
+    const uint32_t r = jobs[k], w = ns[r];
+    const bool written = w != 0xFFFFFFFFu;
+    if (written) nsubs[k] = (int32_t)(w & 0x7FFFFFFFu);
+    if (outcome[k] == 3) {
+      if (written) throw Err{"dada2b_test_bound: a handed-back job was aligned"};
+      continue;
+    }
+    if (!written) throw Err{"dada2b_test_bound: a job was neither aligned nor handed back"};
+    if (which == 0) { if (outcome[k] < 0) outcome[k] = 0; continue; }      // k_nwrow<BOUND> writes the bare count
+    const bool passed = (w & 0x80000000u) != 0;
+    if (which == 2 && passed != (outcome[k] == 1)) throw Err{"dada2b_test_bound: k_nwfwd's survivor list and its bound decision disagree"};
+    if (which != 2 && outcome[k] == 4 && !passed) throw Err{"dada2b_test_bound: a job that failed the bound was stored"};
+    if (outcome[k] < 0) outcome[k] = passed ? 5 : 0;
+  }
+  for (size_t r = 0; r < n; r++) e_after[r] = E2[r];
+  counters[0] = (int64_t)hc[2]; counters[1] = (int64_t)hc[3]; counters[2] = (int64_t)hc[1]; counters[3] = (int64_t)nstored;
+}
+
 // The k-mer screen of one round (include/dada2b_test.h): Run::launch_screen, the round's own launch sequence, for shard (rank, world)
 // with the bitmaps of that shard built into this call's Run; the per-raw decision is read back from the gapless / NW lists.
 static void do_test_screen(dada2b_ctx *cx, uint32_t centre, const dada2b_opts *o, double kdist_cutoff, uint32_t centre_reads, const uint8_t *lock,
@@ -1890,6 +2033,19 @@ int dada2b_test_pairs(dada2b_ctx *ctx, int32_t npairs, const uint32_t *centre, c
 int dada2b_test_loop_nw(dada2b_ctx *ctx, int32_t which, int32_t npairs, const uint32_t *centre, const uint32_t *raw, const double *err,
                         int32_t Q, const dada2b_opts *opts, double *lambda, int32_t *nsubs, int32_t *handled, char errbuf[DADA2B_ERRLEN]) {
   try { do_test_loop_nw(ctx, which, npairs, centre, raw, err, Q, opts, lambda, nsubs, handled); return 0; }
+  catch (Err &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.msg.c_str()); return 1; }
+  catch (std::exception &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.what()); return 2; }
+}
+int dada2b_test_raw_bounds(dada2b_ctx *ctx, const double *err, int32_t Q, int32_t use_quals, int32_t rank, int32_t world, double *S, double *rho,
+                           char errbuf[DADA2B_ERRLEN]) {
+  try { do_test_raw_bounds(ctx, err, Q, use_quals, rank, world, S, rho); return 0; }
+  catch (Err &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.msg.c_str()); return 1; }
+  catch (std::exception &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.what()); return 2; }
+}
+int dada2b_test_bound(dada2b_ctx *ctx, int32_t which, uint32_t centre, uint32_t cluster_i, int64_t njobs, const uint32_t *jobs, const double *e_minmax,
+                      const double *err, int32_t Q, const dada2b_opts *opts, uint64_t njobs_hint, int32_t *outcome, int32_t *nsubs, double *lambda,
+                      double *e_after, int64_t *counters, char errbuf[DADA2B_ERRLEN]) {
+  try { do_test_bound(ctx, which, centre, cluster_i, njobs, jobs, e_minmax, err, Q, opts, njobs_hint, outcome, nsubs, lambda, e_after, counters); return 0; }
   catch (Err &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.msg.c_str()); return 1; }
   catch (std::exception &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.what()); return 2; }
 }

@@ -77,6 +77,8 @@ struct FwdArgs {
   uint32_t *surv_list;
   unsigned long long *surv_count;
   int no_cells;                         // pass 2 of the two-phase scheme: the bound pass already counted these pairs' DP cells
+  uint32_t *ns_out;                     // test hook only (NULL in the product path): nsubs per raw of the bound-testing loop kernels,
+                                        // bit 31 set when the pair passed the bound (k_nwlane, k_nwfwd's bound pass, k_gapless_loop)
 };
 bool launch_nwfwd(const FwdArgs &a, int slots_needed, unsigned long long njobs_upper, unsigned long long njobs_hint, int num_sms, cudaStream_t s,
                   bool bound_only = false);

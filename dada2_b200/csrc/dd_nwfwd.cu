@@ -346,6 +346,7 @@ __global__ void __launch_bounds__(128) k_nwfwd(FwdArgs a) {
         const double bound = a.raw_S[r] * pow(a.raw_rho[r], (double)(ns & (GAPFLAG - 1))) * (double)a.total_reads * (1.0 + 1e-9);
         survive = !(bound <= a.st.E_minmax[r]) || bound < 1e-280;     // near underflow the fp product is not a safe bound: keep
       }
+      if (owner && a.ns_out) a.ns_out[r] = (uint32_t)(ns & (GAPFLAG - 1)) | (survive ? 0x80000000u : 0u);
       const unsigned ms = __ballot_sync(0xffffffffu, survive);
       unsigned long long bs = 0;
       if (lane == 0 && ms) bs = atomicAdd(a.surv_count, (unsigned long long)__popc(ms));

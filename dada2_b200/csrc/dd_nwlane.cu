@@ -179,6 +179,7 @@ __global__ void __launch_bounds__(128) k_nwlane(LaneArgs la) {
       const double bound = a.raw_S[r] * pow(a.raw_rho[r], (double)ns) * (double)a.total_reads * (1.0 + 1e-9);
       survive = !(bound <= a.st.E_minmax[r]) || bound < 1e-280;
     }
+    if (owner && a.ns_out) a.ns_out[r] = (uint32_t)ns | (survive ? 0x80000000u : 0u);
     if (owner && !a.no_cells) cells_lane += cells_pair;
     // Every main-diagonal cell took the diagonal move strictly: the traced path is the gapless alignment (DESIGN.md 4.2), no walk
     // needed -- and its lambda is formed by the whole lane group: lane g looks up the factor of position p0 + g (bases, quality,

@@ -245,10 +245,13 @@ __global__ void __launch_bounds__(128) k_gapless_loop(FwdArgs a, int use_bound) 
       if (left < 16) mis &= (1u << (2 * left)) - 1u;
       ns += __popc(mis);
     }
+    bool survive = true;
     if (use_bound && a.cluster_i != 0) {               // lambda <= S_r * rho_r^nsubs (dd_round.cu:k_raw_bounds): unstorable pairs stop here
       const double bound = a.raw_S[r] * pow(a.raw_rho[r], (double)ns) * (double)a.total_reads * (1.0 + 1e-9);
-      if (bound <= a.st.E_minmax[r] && !(bound < 1e-280)) continue;
+      survive = !(bound <= a.st.E_minmax[r]) || bound < 1e-280;
     }
+    if (a.ns_out) a.ns_out[r] = (uint32_t)ns | (survive ? 0x80000000u : 0u);
+    if (!survive) continue;
     const uint8_t *qrow = a.in.qual + (size_t)r * a.in.QS;
     double lam = 1.0;
     uint4 qn = *(const uint4 *)qrow;

@@ -47,6 +47,25 @@ int dada2b_test_screen(dada2b_ctx *ctx, uint32_t centre, const dada2b_opts *opts
                        const uint8_t *lock, int32_t rank, int32_t world, int32_t max_sms, int32_t path, int32_t *kind, int32_t *minsum,
                        int64_t *counters, char errbuf[DADA2B_ERRLEN]);
 
+/* Per-raw factors of the two-phase loop NW's bound (DESIGN.md 9.3): k_raw_bounds for the raws r with r % world == rank, as a run
+ * launches it.  S[r] = product over the raw's positions of its self-transition factor, rho[r] = largest substitution / self ratio at
+ * the raw's (base, quality) positions; nraw entries each, NaN for the raws of other ranks. */
+int dada2b_test_raw_bounds(dada2b_ctx *ctx, const double *err, int32_t Q, int32_t use_quals, int32_t rank, int32_t world, double *S, double *rho,
+                           char errbuf[DADA2B_ERRLEN]);
+
+/* Stage hook for the bound pass of a round: ONE launch of one bound-testing loop kernel over the job list jobs[njobs] (distinct raws)
+ * against `centre`, as cluster `cluster_i` >= 1 compares them, with E_minmax[r] = e_minmax[r] (nraw entries) going in:
+ *   which = 0  k_nwrow<BOUND>   (no lane-size early return)       which = 2  k_nwfwd, bound pass (njobs_hint picks the instantiation)
+ *   which = 1  k_nwlane (njobs <= its lane_max)                     which = 3  k_gapless_loop with the bound
+ * Per job: outcome 0 dropped by the bound, 1 in the survivor list, 2 in the gapless list (diagonal survivor of k_nwrow<BOUND>),
+ * 3 handed back (length differs / band does not fit), 4 stored, 5 passed the bound but the store rule did not store it;
+ * nsubs (-1 if not aligned); lambda (the stored lambda, NaN if not stored).  e_after: E_minmax after the launch (nraw entries).
+ * counters: survivors listed, gapless-listed, handed back, stored.  Fails when a raw appears twice over the lists, a list holds a raw
+ * that is no job, or a count is out of range. */
+int dada2b_test_bound(dada2b_ctx *ctx, int32_t which, uint32_t centre, uint32_t cluster_i, int64_t njobs, const uint32_t *jobs, const double *e_minmax,
+                      const double *err, int32_t Q, const dada2b_opts *opts, uint64_t njobs_hint, int32_t *outcome, int32_t *nsubs, double *lambda,
+                      double *e_after, int64_t *counters, char errbuf[DADA2B_ERRLEN]);
+
 #ifdef __cplusplus
 }
 #endif

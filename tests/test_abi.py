@@ -28,7 +28,7 @@ def test_library_exports_every_declared_symbol():
         src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
         names |= set(re.findall(r"\b(dada2b_[a-z_A-Z0-9]+)\s*\(", src))
     assert {"dada2b_run", "dada2b_free", "dada2b_upload", "dada2b_run_resident", "dada2b_ctx_free",
-            "dada2b_default_opts", "dada2b_test_pairs", "dada2b_test_calc_pA", "dada2b_test_screen", "dada2b_table_bimera", "dada2b_is_bimera",
+            "dada2b_default_opts", "dada2b_test_pairs", "dada2b_test_calc_pA", "dada2b_test_screen", "dada2b_test_raw_bounds", "dada2b_test_bound", "dada2b_table_bimera", "dada2b_is_bimera",
             "dada2b_bimera_default_opts", "dada2b_test_bimera_pairs", "dada2b_merge_pairs", "dada2b_merge_free",
             "dada2b_merge_default_opts", "dada2b_derep", "dada2b_derep_free", "dada2b_derep_resident"} <= names
     for n in sorted(names):
