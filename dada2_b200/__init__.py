@@ -17,3 +17,5 @@ from . import denoise  # noqa: F401,E402
 from .denoise import dada, learnErrors  # noqa: F401,E402
 from . import taxonomy  # noqa: F401,E402
 from .taxonomy import TaxDB, assignTaxonomy  # noqa: F401,E402
+from . import species  # noqa: F401,E402
+from .species import SpeciesDB, addSpecies, assignSpecies  # noqa: F401,E402
