@@ -45,7 +45,7 @@ def lib():
                                         C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_int32, C.c_char_p]
         L.dada2b_test_loop_nw.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, P(_abi.Opts),
-                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p]
+                                          C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p]
         L.dada2b_test_screen.argtypes = [C.c_void_p, C.c_uint32, P(_abi.Opts), C.c_double, C.c_uint32, C.c_void_p, C.c_int32, C.c_int32,
                                          C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p]
         L.dada2b_test_raw_bounds.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
@@ -157,9 +157,10 @@ class Resident:
             raise Dada2bError(eb.value.decode())
         return dict(kind=kind, lam=lam, nsubs=nsubs, ops=ops, nops=nops, pos=pos, nt0=nt0, nt1=nt1, q1=q1)
 
-    def test_loop_nw(self, which, centre, raw, err, **opts):
+    def test_loop_nw(self, which, centre, raw, err, njobs_hint=1, **opts):
         """Kernel-level hook (include/dada2b_test.h): each (centre, raw) pair alone through one loop aligner
-        (0 k_nwrow<EXACT>, 1 k_nwlane, 2 k_nwfwd, 3 k_nwrow<BOUND>) -> lambda, nsubs, handled."""
+        (0 k_nwrow<EXACT>, 1 k_nwlane, 2 k_nwfwd, 3 k_nwrow<BOUND>) -> lambda, nsubs, handled.  njobs_hint: the round size
+        k_nwfwd picks its instantiation from (1: the small-round choice; above num_sms * 512 the G = 4 / ND = 10 kernel)."""
         e = _check_err(err)
         ecm = np.asfortranarray(e)
         o = _abi.make_opts(**_normalise_opts(dict(opts)))
@@ -169,7 +170,7 @@ class Resident:
         lam = np.zeros(n, np.float64); nsubs = np.zeros(n, np.int32); handled = np.zeros(n, np.int32)
         eb = C.create_string_buffer(_abi.ERRLEN)
         rc = lib().dada2b_test_loop_nw(self._ctx, int(which), n, centre.ctypes.data, raw.ctypes.data, ecm.ctypes.data, int(e.shape[1]),
-                                       C.byref(o), lam.ctypes.data, nsubs.ctypes.data, handled.ctypes.data, eb)
+                                       C.byref(o), int(njobs_hint), lam.ctypes.data, nsubs.ctypes.data, handled.ctypes.data, eb)
         if rc:
             raise Dada2bError(eb.value.decode())
         return dict(lam=lam, nsubs=nsubs, handled=handled)

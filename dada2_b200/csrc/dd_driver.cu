@@ -1767,7 +1767,7 @@ static void do_test_pairs(dada2b_ctx *cx, int npairs, const uint32_t *centre, co
 // Loop aligners one pair at a time (include/dada2b_test.h): the pair is compared as cluster 0 would (E_minmax = -999: always
 // stored, slot = raw index), so (lambda, hamming) can be read back from the comparison store.
 static void do_test_loop_nw(dada2b_ctx *cx, int which, int npairs, const uint32_t *centre, const uint32_t *raw, const double *err_cm, int Q,
-                            const dada2b_opts *o, double *lambda, int32_t *nsubs, int32_t *handled) {
+                            const dada2b_opts *o, uint64_t njobs_hint, double *lambda, int32_t *nsubs, int32_t *handled) {
   CK(cudaSetDevice(cx->device));
   if (cx->bad_nt) throw Err{"Unexpected nucleotide."};
   Run R;
@@ -1802,7 +1802,7 @@ static void do_test_loop_nw(dada2b_ctx *cx, int which, int npairs, const uint32_
     bool launched = false;
     if (which == 0 && R.row_mv.p) launched = launch_nwrow_exact(f, uneq.p, cnt.p + 1, R.row_mv.p, R.row_sub.p, (int)cx->len[c], 1, R.row_grid_cap, s);
     else if (which == 1 && R.lane_mv.p) launched = launch_nwlane(f, uneq.p, cnt.p + 1, R.lane_mv.p, R.lane_sub.p, (int)cx->len[c], R.lane_max, (int)R.lane_max, s);
-    else if (which == 2 && R.P.band >= 0) launched = launch_nwfwd(f, R.fwd_slots, 1, 1, cx->num_sms, s);
+    else if (which == 2 && R.P.band >= 0) launched = launch_nwfwd(f, R.fwd_slots, 1, njobs_hint, cx->num_sms, s);
     else if (which == 3 && R.row_mv.p && R.two_phase) launched = launch_nwrow_bound(f, uneq.p, cnt.p + 1, (int)cx->len[c], 1, cx->num_sms, 0ull, s, nsb.p);
     if (!launched) continue;
     unsigned long long hc[3]; double lam; uint32_t ham, nsv;
@@ -2031,8 +2031,9 @@ int dada2b_test_pairs(dada2b_ctx *ctx, int32_t npairs, const uint32_t *centre, c
   catch (std::exception &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.what()); return 2; }
 }
 int dada2b_test_loop_nw(dada2b_ctx *ctx, int32_t which, int32_t npairs, const uint32_t *centre, const uint32_t *raw, const double *err,
-                        int32_t Q, const dada2b_opts *opts, double *lambda, int32_t *nsubs, int32_t *handled, char errbuf[DADA2B_ERRLEN]) {
-  try { do_test_loop_nw(ctx, which, npairs, centre, raw, err, Q, opts, lambda, nsubs, handled); return 0; }
+                        int32_t Q, const dada2b_opts *opts, uint64_t njobs_hint, double *lambda, int32_t *nsubs, int32_t *handled,
+                        char errbuf[DADA2B_ERRLEN]) {
+  try { do_test_loop_nw(ctx, which, npairs, centre, raw, err, Q, opts, njobs_hint, lambda, nsubs, handled); return 0; }
   catch (Err &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.msg.c_str()); return 1; }
   catch (std::exception &e) { snprintf(errbuf, DADA2B_ERRLEN, "%s", e.what()); return 2; }
 }

@@ -30,9 +30,13 @@ int dada2b_test_calc_pA(int32_t n, const int32_t *reads, const double *E, const 
  *   which = 1  k_nwlane         lane group per pair, software-pipelined rows        (dd_nwlane.cu)
  *   which = 2  k_nwfwd          lane-group anti-diagonal wavefront, carried lambda  (dd_nwfwd.cu)
  *   which = 3  k_nwrow<BOUND>   thread per pair, substitution count only (lambda[k] is left 0)
- * handled[k] = 0 when the kernel does not take the pair (lengths differ, band not instantiated, ...) and hands it on. */
+ * njobs_hint is the round size k_nwfwd picks its instantiation from, as in a run (above num_sms * 512: the "big" G = 4 / ND = 10
+ * kernel for the narrowest slot class); the other kernels ignore it.
+ * handled[k] = 0 when the kernel does not take the pair (lengths differ, band not instantiated, shared memory too small, ...) and
+ * hands it on. */
 int dada2b_test_loop_nw(dada2b_ctx *ctx, int32_t which, int32_t npairs, const uint32_t *centre, const uint32_t *raw, const double *err,
-                        int32_t Q, const dada2b_opts *opts, double *lambda, int32_t *nsubs, int32_t *handled, char errbuf[DADA2B_ERRLEN]);
+                        int32_t Q, const dada2b_opts *opts, uint64_t njobs_hint, double *lambda, int32_t *nsubs, int32_t *handled,
+                        char errbuf[DADA2B_ERRLEN]);
 
 /* Stage hook for the k-mer screen of one round (raw_align's shroud / gapless / NW decision, nwalign_endsfree.cpp:44-56, with the
  * greedy skip of cluster.cpp:127-131): centre `centre` against every raw r with r % world == rank, through the round's own launch

@@ -35,6 +35,30 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(L, n), "libdada2b.so does not export %s" % n
 
 
+_CTYPE_OF = {"int32_t": "c_int", "uint32_t": "c_uint", "int64_t": "c_long", "uint64_t": "c_ulong", "double": "c_double"}
+
+
+def test_test_hook_bindings_match_header():
+    """Every stage hook of include/dada2b_test.h is bound in api.lib() with one ctypes argument per C parameter, of the same kind:
+    a pointer where the header has one, an integer of the same width and sign, a double.  A parameter added to a hook (njobs_hint
+    of dada2b_test_loop_nw, dada2b_test_bound) without its binding would shift every later argument."""
+    L = _lib()
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "dada2b_test.h")).read(), flags=re.S)
+    protos = re.findall(r"\bint\s+(dada2b_test_\w+)\s*\(([^)]*)\)\s*;", src)
+    assert {n for n, _ in protos} >= {"dada2b_test_pairs", "dada2b_test_loop_nw", "dada2b_test_bound", "dada2b_test_raw_bounds"}
+    for name, params in protos:
+        params = [" ".join(p.split()) for p in params.split(",")]
+        argt = getattr(L, name).argtypes
+        assert argt is not None and len(argt) == len(params), (name, len(params), argt and len(argt))
+        for p, t in zip(params, argt):
+            if "*" in p or "[" in p:
+                assert t is ctypes.c_void_p or t is ctypes.c_char_p or hasattr(t, "contents"), (name, p, t)
+            else:
+                ct = p.replace("const ", "").split()[0]
+                assert t.__name__ == _CTYPE_OF[ct] or ctypes.sizeof(t) == ctypes.sizeof(getattr(ctypes, _CTYPE_OF[ct])) and \
+                    (t.__name__.startswith("c_u") == _CTYPE_OF[ct].startswith("c_u")), (name, p, t)
+
+
 def test_struct_layouts_match_ctypes_mirror():
     from dada2_b200 import _abi
     prog = r'''
