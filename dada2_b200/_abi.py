@@ -49,13 +49,16 @@ class Out(C.Structure):
                 ("n_k_align_final", C.c_int32),
                 ("ms_k_prescreen", C.c_double), ("ms_k_nw_bound", C.c_double), ("ms_k_nw_exact", C.c_double), ("ms_k_tail", C.c_double),
                 ("n_k_prescreen", C.c_int32), ("n_k_nw_bound", C.c_int32), ("n_k_nw_exact", C.c_int32), ("n_k_tail", C.c_int32),
-                ("prescreen_rows", C.c_int64)]
+                ("prescreen_rows", C.c_int64),
+                ("ms_k_final_row", C.c_double), ("ms_k_final_diag", C.c_double), ("ms_k_final_gapped", C.c_double),
+                ("n_k_final_row", C.c_int32), ("n_k_final_diag", C.c_int32), ("n_k_final_gapped", C.c_int32)]
 
 STAT_FIELDS = ["n_align", "n_shroud", "n_nw", "n_gapless", "nw_cells", "n_final_nw", "n_rounds", "n_shuffles",
                "gpu_launches", "h2d_bytes", "d2h_bytes", "ms_setup", "ms_loop", "ms_final", "ms_total", "ms_device",
                "ms_k_classify", "ms_k_align_nw", "ms_k_align_gl", "ms_k_align_final", "n_k_classify", "n_k_align_nw",
                "n_k_align_gl", "n_k_align_final", "ms_k_prescreen", "ms_k_nw_bound", "ms_k_nw_exact", "ms_k_tail", "n_k_prescreen",
-               "n_k_nw_bound", "n_k_nw_exact", "n_k_tail", "prescreen_rows"]
+               "n_k_nw_bound", "n_k_nw_exact", "n_k_tail", "prescreen_rows", "ms_k_final_row", "ms_k_final_diag",
+               "ms_k_final_gapped", "n_k_final_row", "n_k_final_diag", "n_k_final_gapped"]
 
 
 # R/dada.R:1-26 defaults, in dada_uniques argument order (R/dada.R:340-352)

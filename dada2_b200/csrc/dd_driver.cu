@@ -524,6 +524,7 @@ struct Run {
   DBuf<unsigned long long> win_buf, fin_dcount, fin_dall;
   DBuf<uint8_t> fin_cq, fin_rep_d;
   DBuf<uint32_t> fin_rep_rows;
+  DBuf<uint32_t> ft_off, ft_chk, ft_cur, ft_ord, ft_sums;   // k_final_tally's per-cluster offsets and cluster-ordered raws (dd_final.cu)
   PBuf<uint8_t> fin_rep_h;          // representative sequences of the clusters: row list up, packed rows back
   DBuf<double> fin_sv, fin_gv;
   bool prescreen = false;
@@ -589,7 +590,8 @@ struct Run {
   struct Ev { cudaEvent_t a, b; int tag; };
   std::vector<Ev> evs;
   cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
-  enum { T_CLASSIFY = 0, T_NW, T_GL, T_FINAL, T_NWB, T_PRE, T_TAIL, T_N };
+  // final pass: T_FROW = k_nwrow<FINAL> / k_nwfwd (nsubs + path class), T_FDIAG = the diagonal list, T_FGAP = the gapped list
+  enum { T_CLASSIFY = 0, T_NW, T_GL, T_FROW, T_FDIAG, T_FGAP, T_NWB, T_PRE, T_TAIL, T_N };
   long long prescreen_rows = 0;
   template <typename F> void timed(int tag, F f) {
     Ev e{cx->get_event(), cx->get_event(), tag};
@@ -917,8 +919,11 @@ void Run::launch_compare(uint32_t i, double kdist_cutoff) {
       const long worst = (long)in.maxlen * std::max(std::abs(P.mismatch), std::abs(P.match)) + std::max(std::abs(P.gap), std::abs(P.hgap)) + 16;
       f.fast_ok = (worst < std::abs((long)P.sentinel) / 2) ? 1 : 0;
     }
-    if (two_phase && i > 0 && !P.homo) {
-      // pass 1: scores + substitution counts only; lambda <= S_r * rho_r^nsubs decides which pairs can pass the store rule
+    const unsigned long long fwd_hint = i == 0 ? (unsigned long long)nraw : est_active;
+    if (two_phase && !P.homo) {
+      // pass 1: scores + substitution counts only; lambda <= S_r * rho_r^nsubs decides which pairs can pass the store rule.
+      // Round 0 (E_minmax still -999, containers.cpp:39) keeps every pair, but its diagonal-path pairs still leave for
+      // k_gapless_loop, so that only real gaps reach the exact pass
       FwdArgs fbnd = f;
       fbnd.raw_S = raw_S.p; fbnd.raw_rho = raw_rho.p; fbnd.surv_list = surv_list.p; fbnd.surv_count = st.ctr + CTR_SURV;
       if (!fallback_only) { fbnd.gl_out = st.gl_list; fbnd.gl_count = st.ctr + CTR_GL; }   // diagonal-path survivors -> k_gapless_loop
@@ -931,7 +936,7 @@ void Run::launch_compare(uint32_t i, double kdist_cutoff) {
       if (done_row) { fbnd.jobs = uneq_list.p; fbnd.njobs_ptr = st.ctr + CTR_UNEQ_B; }
       bool done_rest = done_row && in.minlen == in.maxlen;          // every raw has the centre's length: nothing was handed back
       if (!done_rest)
-        timed(T_NWB, [&]() { done_rest = launch_nwfwd(fbnd, fwd_slots, (unsigned long long)nraw, done_row ? 0 : est_active, cx->num_sms, s, true); fb_possible |= done_rest; });
+        timed(T_NWB, [&]() { done_rest = launch_nwfwd(fbnd, fwd_slots, (unsigned long long)nraw, done_row ? 0 : fwd_hint, cx->num_sms, s, true); fb_possible |= done_rest; });
       // pass 2: the exact forward-carry kernel on the survivors
       if (done_rest) { f.jobs = surv_list.p; f.njobs_ptr = st.ctr + CTR_SURV; f.no_cells = 1; }
     }
@@ -951,7 +956,7 @@ void Run::launch_compare(uint32_t i, double kdist_cutoff) {
       if (ex_done) { f.jobs = uneq_list.p; f.njobs_ptr = st.ctr + CTR_UNEQ_X; }
     }
     if (ex_done && in.minlen == in.maxlen) fwd_done = true;       // nothing was handed back; fb_list stays empty
-    else timed(T_NW, [&]() { fwd_done = launch_nwfwd(f, fwd_slots, (unsigned long long)nraw, ex_done ? 0 : (i == 0 ? (unsigned long long)nraw : est_active), cx->num_sms, s); fb_possible |= fwd_done; });
+    else timed(T_NW, [&]() { fwd_done = launch_nwfwd(f, fwd_slots, (unsigned long long)nraw, ex_done ? 0 : fwd_hint, cx->num_sms, s); fb_possible |= fwd_done; });
   }
   if (!fallback_only) {       // gapless comparisons: no DP, one thread per pair (dd_nwrow.cu:k_gapless_loop)
     FwdArgs g{};
@@ -1298,7 +1303,12 @@ template <typename T> T *dupv(const std::vector<T> &v) {
 
 // Rmain.cpp:168-295: final subs, final p, output tables
 void Run::finish(dada2b_out *out) {
+  // DADA2B_VERBOSE: host clock per phase; the device work of a phase is waited for before its end is read
+  const bool vb = getenv("DADA2B_VERBOSE") != nullptr;
+  double ph[7]; int nph = 0;
+  ph[nph++] = now_ms();
   drain_replay();
+  ph[nph++] = now_ms();
   const uint32_t nclust = (uint32_t)members.size();
   const int maxlen = in.maxlen;
   if (pending.apply) { launch_round_begin(st, 1, pending.r, pending.from, pending.newi, pending.reads, s); pending.apply = 0; }
@@ -1308,8 +1318,8 @@ void Run::finish(dada2b_out *out) {
   st.trans = trans.p; st.cq_sum = cq_sum.p; st.cq_cnt = cq_cnt.p;
   const int n_owned = (nraw - cx->rank + cx->world - 1) / cx->world;     // raws aligned by this rank in the final pass
   if (cx->world > 1) nsubs_final.zero(s);
+  bool split = false;                    // the raws are split into a diagonal and a gapped list
   {  // FinalSubsParallel: sub_new(centre, raw, use_kmers=false) for every raw
-    bool split = false;
     if (P.band > 0) {
       // 1) forward-carry NW of every raw against its own centre: nsubs + "is the optimal path the pure diagonal?"
       FwdArgs f{};
@@ -1326,25 +1336,37 @@ void Run::finish(dada2b_out *out) {
       bool row_done = false;
       if (row_mv.p) {       // thread-per-pair row kernel when every sequence has the same length (dd_nwrow.cu), else the lane-group kernel
         CK(cudaMemsetAsync(uneq_ctr.p, 0, 8, s));
-        timed(T_FINAL, [&]() { row_done = launch_nwrow_final(f, uneq_list.p, uneq_ctr.p, (unsigned long long)nraw, cx->num_sms, s); });
+        timed(T_FROW, [&]() { row_done = launch_nwrow_final(f, uneq_list.p, uneq_ctr.p, (unsigned long long)nraw, cx->num_sms, s); });
       }
       if (row_done) split = true;
-      else timed(T_FINAL, [&]() { split = launch_nwfwd(f, fwd_slots, (unsigned long long)nraw, (unsigned long long)nraw, cx->num_sms, s); });
+      else timed(T_FROW, [&]() { split = launch_nwfwd(f, fwd_slots, (unsigned long long)nraw, (unsigned long long)nraw, cx->num_sms, s); });
     }
     if (split) {
-      // 2) gapless column list for the pure-diagonal pairs, 3) traceback kernel for the rest (+ pairs that did not fit)
-      for (int pass = 0; pass < 3; pass++) {
-        AlignArgs a = align_args(MODE_FINAL, pass == 0 ? KIND_GAPLESS : KIND_NW);
-        a.jobs = pass == 0 ? st.gl_list : (pass == 1 ? st.nw_list : fb_list.p);
-        a.njobs_ptr = st.ctr + (pass == 0 ? CTR_GL : (pass == 1 ? CTR_NW : CTR_NMOVE));
-        timed(T_FINAL, [&]() { launch_align_jobs(MODE_FINAL, a, (unsigned long long)nraw); });
+      // 2) per-cluster reduction over the pure-diagonal raws (dd_final.cu), 3) traceback kernel for the rest (+ pairs that did not fit)
+      ft_off.alloc((size_t)nclust + 1); ft_chk.alloc((size_t)nclust + 1); ft_cur.alloc(nclust); ft_ord.alloc(std::max(n_owned, 1));
+      ft_sums.alloc(final_tally_scan_words((int)nclust));
+      ft_off.zero(s);
+      timed(T_FDIAG, [&]() {
+        launch_final_tally(in, st, st.gl_list, st.ctr + CTR_GL, (unsigned long long)n_owned, (int)nclust, ncol, ft_off.p, ft_chk.p, ft_cur.p, ft_ord.p,
+                           ft_sums.p, cx->num_sms, s);
+      });
+      for (int pass = 1; pass < 3; pass++) {
+        AlignArgs a = align_args(MODE_FINAL, KIND_NW);
+        a.jobs = pass == 1 ? st.nw_list : fb_list.p;
+        a.njobs_ptr = st.ctr + (pass == 1 ? CTR_NW : CTR_NMOVE);
+        timed(T_FGAP, [&]() { launch_align_jobs(MODE_FINAL, a, (unsigned long long)nraw); });
       }
     } else {
       AlignArgs a = align_args(MODE_FINAL, P.band == 0 ? KIND_GAPLESS : KIND_NW);
       a.jobs = nullptr; a.njobs_ptr = nullptr; a.njobs_fixed = n_owned; a.job_mul = cx->world; a.job_add = cx->rank;
-      timed(T_FINAL, [&]() { launch_align_jobs(MODE_FINAL, a, (unsigned long long)nraw); });
+      timed(T_FGAP, [&]() { launch_align_jobs(MODE_FINAL, a, (unsigned long long)nraw); });
     }
   }
+  if (vb) {
+    read_ctr();                            // synchronises
+    if (split) fprintf(stderr, "[dada2b] final pass lists: diagonal %llu, gapped %llu, handed back %llu\n", h_ctr.p[CTR_GL], h_ctr.p[CTR_NW], h_ctr.p[CTR_NMOVE]);
+  }
+  ph[nph++] = now_ms();
   if (cx->world > 1) {   // every rank tallied its own raws: integer sums are exact and order-independent
     NC(g_nccl.AllReduce(trans.p, trans.p, (size_t)16 * ncol, ncclInt32, ncclSum, cx->comm, s));
     NC(g_nccl.AllReduce(cq_sum.p, cq_sum.p, (size_t)nclust * maxlen, ncclUint64, ncclSum, cx->comm, s));
@@ -1404,6 +1426,7 @@ void Run::finish(dada2b_out *out) {
     d2h(bq1.data(), b_q1.p, bq1.size());
     sync();
   }
+  ph[nph++] = now_ms();
   // post-hoc cluster p-values (error.cpp:99-119)
   std::vector<double> tot_e(nclust, 0.0), cpval(nclust, 0.0);
   {
@@ -1469,6 +1492,8 @@ void Run::finish(dada2b_out *out) {
     launch_calc_pA_vec(pa_reads.p, pa_E.p, pa_prior.p, pa_out.p, (int)nclust, s);
     d2h(cpval.data(), pa_out.p, nclust * 8);
   }
+  if (vb) sync();
+  ph[nph++] = now_ms();
   // per-raw results: staged in the pinned arena and written straight into the output arrays by several threads
   std::vector<int> htrans((size_t)16 * ncol); std::vector<unsigned long long> hsum((size_t)nclust * maxlen), hcnt((size_t)nclust * maxlen);
   d2h(htrans.data(), trans.p, htrans.size() * 4);
@@ -1482,6 +1507,7 @@ void Run::finish(dada2b_out *out) {
   const uint8_t *hcorrect = stage(correct.p, nraw);
   read_ctr();                                     // synchronises; nothing below touches the arena
   check_dev_error();
+  ph[nph++] = now_ms();
 
   out->nclust = nclust; out->nraw = nraw; out->maxlen = maxlen; out->Q = ncol;
   out->n_align = (int64_t)h_ctr.p[CTR_ALIGN]; out->n_shroud = (int64_t)h_ctr.p[CTR_SHROUD];
@@ -1589,19 +1615,24 @@ void Run::finish(dada2b_out *out) {
   float ms = 0;
   CK(cudaEventElapsedTime(&ms, ev_begin, ev_end));
   out->ms_device = ms;
-  double sum[T_N] = {0, 0, 0, 0, 0, 0, 0}; int cnt[T_N] = {0, 0, 0, 0, 0, 0, 0};
+  double sum[T_N] = {}; int cnt[T_N] = {};
   for (const Ev &e : evs) { float t = 0; if (cudaEventElapsedTime(&t, e.a, e.b) == cudaSuccess) { sum[e.tag] += t; cnt[e.tag]++; } }
   if (getenv("DADA2B_VERBOSE")) fprintf(stderr, "[dada2b] loop NW: bound pass %.3f ms (%d launches), exact %.3f ms (%d launches)\n", sum[T_NWB], cnt[T_NWB], sum[T_NW], cnt[T_NW]);
   out->ms_k_prescreen = sum[T_PRE]; out->n_k_prescreen = cnt[T_PRE]; out->prescreen_rows = prescreen_rows;
   out->ms_k_nw_bound = sum[T_NWB]; out->n_k_nw_bound = cnt[T_NWB]; out->ms_k_nw_exact = sum[T_NW]; out->n_k_nw_exact = cnt[T_NW];
   out->ms_k_tail = sum[T_TAIL]; out->n_k_tail = cnt[T_TAIL];
+  out->ms_k_final_row = sum[T_FROW]; out->ms_k_final_diag = sum[T_FDIAG]; out->ms_k_final_gapped = sum[T_FGAP];
+  out->n_k_final_row = cnt[T_FROW]; out->n_k_final_diag = cnt[T_FDIAG]; out->n_k_final_gapped = cnt[T_FGAP];
   sum[T_NW] += sum[T_NWB]; cnt[T_NW] += cnt[T_NWB];
   sum[T_CLASSIFY] += sum[T_PRE]; cnt[T_CLASSIFY] += cnt[T_PRE];
-  out->ms_k_classify = sum[T_CLASSIFY]; out->ms_k_align_nw = sum[T_NW]; out->ms_k_align_gl = sum[T_GL]; out->ms_k_align_final = sum[T_FINAL];
-  out->n_k_classify = cnt[T_CLASSIFY]; out->n_k_align_nw = cnt[T_NW]; out->n_k_align_gl = cnt[T_GL]; out->n_k_align_final = cnt[T_FINAL];
+  out->ms_k_classify = sum[T_CLASSIFY]; out->ms_k_align_nw = sum[T_NW]; out->ms_k_align_gl = sum[T_GL]; out->ms_k_align_final = sum[T_FROW] + sum[T_FDIAG] + sum[T_FGAP];
+  out->n_k_classify = cnt[T_CLASSIFY]; out->n_k_align_nw = cnt[T_NW]; out->n_k_align_gl = cnt[T_GL]; out->n_k_align_final = cnt[T_FROW] + cnt[T_FDIAG] + cnt[T_FGAP];
   out->n_final_nw = (P.band == 0) ? 0 : nraw;
   out->gpu_launches = launches_count() - launches0;
   out->h2d_bytes = h2d_bytes; out->d2h_bytes = d2h_bytes;
+  ph[nph++] = now_ms();
+  if (vb) fprintf(stderr, "[dada2b] finish host ms: drain replay %.2f, final pass %.2f, birth subs %.2f, post-hoc %.2f, D2H %.2f, host tallies/output %.2f\n",
+                  ph[1] - ph[0], ph[2] - ph[1], ph[3] - ph[2], ph[4] - ph[3], ph[5] - ph[4], ph[6] - ph[5]);
 }
 
 dada2b_out *do_run(dada2b_ctx *cx, const double *err_cm, int Q, const dada2b_opts *o) {

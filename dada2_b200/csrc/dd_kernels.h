@@ -149,6 +149,13 @@ void launch_round_begin(const DevState &st, int apply, uint32_t r, uint32_t from
 void launch_fill_f64(double *p, double v, size_t n, cudaStream_t s);
 void launch_center_cluster(int *cc, const uint32_t *cl_center, int nclust, cudaStream_t s);
 void launch_final_p(const DevState &st, const DevIn &in, double omegaC, cudaStream_t s);
+// dd_final.cu: final pass, raws whose alignment against their own centre is the main diagonal (list / *count): nsubs_final, and
+// trans / cq_sum / cq_cnt of the correct ones.  Scratch: off and chk [nclust + 1] (off zeroed by the caller), cur [nclust],
+// ord [upper], scan_sums [final_tally_scan_words(nclust)].  upper bounds *count.
+size_t final_tally_scan_words(int nclust);
+void launch_final_tally(const DevIn &in, const DevState &st, const uint32_t *list, const unsigned long long *count, unsigned long long upper,
+                        int nclust, int ncol, uint32_t *off, uint32_t *chk, uint32_t *cur, uint32_t *ord, uint32_t *scan_sums, int num_sms,
+                        cudaStream_t s);
 void launch_calc_pA_vec(const int *reads, const double *E, const int *prior, double *out, int n, cudaStream_t s);
 
 }  // namespace dd2

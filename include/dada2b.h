@@ -104,6 +104,10 @@ typedef struct {
   double ms_k_prescreen, ms_k_nw_bound, ms_k_nw_exact, ms_k_tail;
   int32_t n_k_prescreen, n_k_nw_bound, n_k_nw_exact, n_k_tail;
   int64_t prescreen_rows;           /* 5-mer bitmap rows (128 B + 13 B of per-raw metadata) streamed by k_prescreen */
+  /* final pass split (ms_k_align_final = row + diag + gapped): the sweep that finds nsubs and the path class, the tally of the
+   * raws whose final alignment is the main diagonal, and the traceback alignments of the rest */
+  double ms_k_final_row, ms_k_final_diag, ms_k_final_gapped;
+  int32_t n_k_final_row, n_k_final_diag, n_k_final_gapped;
 } dada2b_out;
 
 /* One-shot: host buffers in, host buffers out (what the Rcpp shim calls). */
