@@ -19,3 +19,5 @@ from . import taxonomy  # noqa: F401,E402
 from .taxonomy import TaxDB, assignTaxonomy  # noqa: F401,E402
 from . import species  # noqa: F401,E402
 from .species import SpeciesDB, addSpecies, assignSpecies  # noqa: F401,E402
+from . import paired  # noqa: F401,E402
+from .paired import mergePairs  # noqa: F401,E402

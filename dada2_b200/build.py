@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdada2b.so")
-SOURCES = ["dd_kernels.cu", "dd_final.cu", "dd_nwfwd.cu", "dd_nwrow.cu", "dd_nwlane.cu", "dd_prescreen.cu", "dd_round.cu", "dd_round2.cu", "dd_driver.cu", "dd_bimera.cu", "dd_bimfwd.cu", "dd_bimfwd16.cu", "dd_merge.cu", "dd_derep.cu", "dd_collapse.cu", "dd_filter.cu", "dd_primer.cu", "dd_pool.cu", "dd_taxonomy.cu", "dd_species.cu"]
+SOURCES = ["dd_kernels.cu", "dd_final.cu", "dd_nwfwd.cu", "dd_nwrow.cu", "dd_nwlane.cu", "dd_prescreen.cu", "dd_round.cu", "dd_round2.cu", "dd_driver.cu", "dd_bimera.cu", "dd_bimfwd.cu", "dd_bimfwd16.cu", "dd_merge.cu", "dd_pairs.cu", "dd_derep.cu", "dd_collapse.cu", "dd_filter.cu", "dd_primer.cu", "dd_pool.cu", "dd_taxonomy.cu", "dd_species.cu"]
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-fmad=false",
          "-Xcompiler", "-fPIC,-O2,-pthread", "-diag-suppress", "550"]
 

@@ -7,9 +7,7 @@
 // One warp per pairing: the warp-per-pair NW with traceback of dd_nw_warp.cuh (unbanded for mergePairs: the move matrix
 // lives in a per-warp global scratch row), then two lane-parallel passes over the alignment columns -- column masks and
 // end-gap runs for the counts, consensus characters written straight to the output row.  Integer / byte work only.
-#include "../../include/dada2b_merge.h"
-#include "dd_evalpair.cuh"
-#include "dd_hostutil.h"
+#include "dd_merge.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -17,20 +15,6 @@
 #include <cstring>
 
 namespace dd2 {
-
-struct MergeArgs {
-  BimSeqs sq;
-  AlnParams P;
-  int trim_overhang;
-  const int32_t *s1_idx, *s2_idx, *prefer;
-  int npairs;
-  int32_t *counts;                 // [npairs][3] match, mismatch, indel
-  char *cons; int cons_stride;     // [npairs][cons_stride]
-  int32_t *cons_len;               // [npairs]
-  unsigned long long *ctr;         // [1] cells, [2] error flag
-  int warp_words, seq_bytes, H_words, ops_words, mask_words, ptr_in_smem;
-  uint32_t *ptr_scratch; unsigned long long ptr_words;
-};
 
 __global__ void __launch_bounds__(128) k_merge_pairs(MergeArgs a) {
   extern __shared__ uint32_t smem[];
@@ -94,6 +78,33 @@ __global__ void __launch_bounds__(128) k_merge_pairs(MergeArgs a) {
   }
 }
 
+void merge_setup(const BimSeqs &sq, const dada2b_merge_opts *opts, int num_sms, int npairs, MergeArgs &a, size_t &smem, int &grid,
+                 BBuf<uint32_t> &d_ptr) {
+  AlnParams &P = a.P;
+  P.match = opts->match; P.mismatch = opts->mismatch; P.gap = opts->gap_p; P.hgap = opts->homo_gap_p; P.band = opts->band;
+  P.homo = opts->gap_p != opts->homo_gap_p ? 1 : 0;                     // evaluate.cpp:40-46
+  P.sentinel = -9999;                                                    // nwalign_endsfree.cpp:116-117
+  const int maxlen = sq.maxlen, minlen = sq.minlen;
+  const int lbmax = P.band < 0 ? maxlen : std::min(P.band + (maxlen - minlen), maxlen), rbmax = lbmax;
+  const int Wmax = lbmax + rbmax + 1;
+  const int nchunk = (((Wmax + 1) >> 1) + 31) >> 5;
+  a.sq = sq;
+  a.seq_bytes = (maxlen + 15) & ~15;
+  a.H_words = (Wmax + 2 + 3) & ~3;
+  a.ops_words = ((2 * maxlen) / 16 + 2 + 3) & ~3;
+  a.mask_words = ((2 * maxlen + 31) / 32 + 2 + 3) & ~3;
+  a.ptr_words = (unsigned long long)(2 * maxlen + 2) * 2 * nchunk;
+  const int base_words = 2 * (a.seq_bytes / 4) + a.H_words + a.ops_words + 3 * a.mask_words;
+  a.ptr_in_smem = (4 * ((size_t)base_words + a.ptr_words) * 4 <= 96 * 1024) ? 1 : 0;
+  a.warp_words = base_words + (a.ptr_in_smem ? (int)a.ptr_words : 0);
+  smem = (size_t)4 * a.warp_words * 4;
+  if (smem > 200 * 1024) throw BErr{"dada2b: band/sequence length too large for the alignment kernel's shared memory."};
+  BCK(cudaFuncSetAttribute(k_merge_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
+  grid = (int)std::min<long long>((long long)num_sms * 8, std::max<long long>(1, ((long long)npairs + 3) / 4));
+  if (!a.ptr_in_smem) { d_ptr.alloc((size_t)grid * 4 * a.ptr_words); a.ptr_scratch = d_ptr.p; }
+  a.trim_overhang = opts->trim_overhang != 0; a.npairs = npairs; a.cons_stride = 2 * maxlen;
+}
+
 }  // namespace dd2
 
 using namespace dd2;
@@ -137,29 +148,9 @@ int dada2b_merge_pairs(int32_t nseq, const char *seq_concat, const int64_t *seq_
     for (int x = 0; x < npairs; x++)
       if (s1_idx[x] < 0 || s1_idx[x] >= nseq || s2_idx[x] < 0 || s2_idx[x] >= nseq) throw BErr{"dada2b: bad pair index."};
     MergeArgs a{};
-    AlnParams &P = a.P;
-    P.match = opts->match; P.mismatch = opts->mismatch; P.gap = opts->gap_p; P.hgap = opts->homo_gap_p; P.band = opts->band;
-    P.homo = opts->gap_p != opts->homo_gap_p ? 1 : 0;                     // evaluate.cpp:40-46
-    P.sentinel = -9999;                                                    // nwalign_endsfree.cpp:116-117
-    const int maxlen = sq.maxlen, minlen = sq.minlen;
-    const int lbmax = P.band < 0 ? maxlen : std::min(P.band + (maxlen - minlen), maxlen), rbmax = lbmax;
-    const int Wmax = lbmax + rbmax + 1;
-    const int nchunk = (((Wmax + 1) >> 1) + 31) >> 5;
-    a.sq = sq;
-    a.seq_bytes = (maxlen + 15) & ~15;
-    a.H_words = (Wmax + 2 + 3) & ~3;
-    a.ops_words = ((2 * maxlen) / 16 + 2 + 3) & ~3;
-    a.mask_words = ((2 * maxlen + 31) / 32 + 2 + 3) & ~3;
-    a.ptr_words = (unsigned long long)(2 * maxlen + 2) * 2 * nchunk;
-    const int base_words = 2 * (a.seq_bytes / 4) + a.H_words + a.ops_words + 3 * a.mask_words;
-    a.ptr_in_smem = (4 * ((size_t)base_words + a.ptr_words) * 4 <= 96 * 1024) ? 1 : 0;
-    a.warp_words = base_words + (a.ptr_in_smem ? (int)a.ptr_words : 0);
-    const size_t smem = (size_t)4 * a.warp_words * 4;
-    if (smem > 200 * 1024) throw BErr{"dada2b: band/sequence length too large for the alignment kernel's shared memory."};
-    BCK(cudaFuncSetAttribute(k_merge_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
-    const int grid = (int)std::min<long long>((long long)num_sms * 8, std::max<long long>(1, ((long long)npairs + 3) / 4));
-    if (!a.ptr_in_smem) { d_ptr.alloc((size_t)grid * 4 * a.ptr_words); a.ptr_scratch = d_ptr.p; }
-    a.trim_overhang = opts->trim_overhang != 0; a.npairs = npairs; a.cons_stride = 2 * maxlen;
+    size_t smem = 0;
+    int grid = 1;
+    merge_setup(sq, opts, num_sms, npairs, a, smem, grid, d_ptr);
     BBuf<int32_t> d_s1, d_s2, d_pref, d_counts, d_clen; BBuf<char> d_cons; BBuf<unsigned long long> d_ctr;
     const size_t np1 = std::max(npairs, 1);
     d_s1.alloc(np1); d_s2.alloc(np1); d_pref.alloc(np1); d_counts.alloc(np1 * 3); d_clen.alloc(np1); d_cons.alloc(np1 * a.cons_stride); d_ctr.alloc(8);

@@ -9,6 +9,7 @@ marshals.  No CPU fallback.
 A table is (mat, colnames, rownames): mat is an int32 [nsample, nseq] matrix like R's seqtab (rows = samples).
 """
 import ctypes as C
+import sys
 
 import numpy as np
 
@@ -128,10 +129,28 @@ def _colsums(mat):
     return cs
 
 
+def _is_merger(s):
+    return isinstance(s, dict) and "clustering" not in s and isinstance(s.get("sequence"), (list, tuple)) and "abundance" in s
+
+
+def _merger_uniques(m):
+    """getUniques' data.frame branch (R/misc.R:42-60): abundance by sequence; duplicated sequences (e.g. the "" of rejected
+    rows kept by returnRejects) are summed with tapply, which sorts the names."""
+    seqs, ab = list(m["sequence"]), [int(a) for a in m["abundance"]]
+    if len(set(seqs)) == len(seqs):
+        return dict(zip(seqs, ab))
+    print("Duplicate sequences detected and merged.", file=sys.stderr)
+    tot = {}
+    for sq, a in zip(seqs, ab):
+        tot[sq] = tot.get(sq, 0) + a
+    return {sq: tot[sq] for sq in sorted(tot)}
+
+
 def makeSequenceTable(samples, orderBy="abundance"):
-    """R/multiSample.R:31-55.  samples: a list of samples, or a dict name -> sample; a sample is a {sequence: count} map or
-    a dada_uniques result (its clustering's sequence / abundance).  -> (int32 mat [nsample, nseq], colnames, rownames)"""
-    if isinstance(samples, dict) and not all(isinstance(v, (dict, list, tuple)) for v in samples.values()):
+    """R/multiSample.R:31-55.  samples: a list of samples, or a dict name -> sample; a sample is a {sequence: count} map,
+    a dada_uniques result (its clustering's sequence / abundance) or a mergePairs merger (its sequence / abundance).
+    -> (int32 mat [nsample, nseq], colnames, rownames)"""
+    if _is_merger(samples) or (isinstance(samples, dict) and not all(isinstance(v, (dict, list, tuple)) for v in samples.values())):
         samples = [samples]
     names = list(samples.keys()) if isinstance(samples, dict) else None
     vals = list(samples.values()) if isinstance(samples, dict) else list(samples)
@@ -140,6 +159,8 @@ def makeSequenceTable(samples, orderBy="abundance"):
         if isinstance(s, dict) and "clustering" in s:                      # getUniques(dada) = clustering's abundance by sequence
             cl = s["clustering"]
             s = dict(zip(cl["sequence"], (int(a) for a in cl["abundance"])))
+        elif _is_merger(s):
+            s = _merger_uniques(s)
         unqs.append(dict(s))
     cols, index = [], {}
     for u in unqs:

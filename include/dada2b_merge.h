@@ -51,6 +51,51 @@ int dada2b_merge_pairs(int32_t nseq, const char *seq_concat, const int64_t *seq_
                        dada2b_merge_out **out, char errbuf[DADA2B_ERRLEN]);
 void dada2b_merge_free(dada2b_merge_out *out);
 
+/* ---- mergePairs over whole samples (R/paired.R:111-197 without the data.frame glue) ----
+ * For S samples: every read's forward / reverse cluster (dadaF$map[mapF], dadaR$map[mapR]; NA propagates and NA reads are
+ * dropped), the unique (forward, reverse) pairings tabulated on the device with their read counts and ordered per sample by
+ * abundance descending, then first occurrence (order(abundance, decreasing = TRUE) over unique()'s rows), prefer =
+ * 1 + (n0R[reverse] > n0F[forward]), one alignment per distinct (forward sequence, reverse sequence, prefer) across all
+ * samples, the accept rule and blanking of rejected consensus sequences.  All maps are 1-based with NA = INT32_MIN.  Cluster
+ * sequences are given as dada() reports them: the reverse ones NOT reverse-complemented (the device does rc()). */
+typedef struct {
+  int32_t nsamples;
+  const int64_t *nreadsF, *nreadsR;       /* [S] reads per sample: lengths of derepF$map and derepR$map                    */
+  const int32_t *mapF, *mapR;             /* derep maps, concatenated sample by sample                                     */
+  const int32_t *nuniqF, *nuniqR;         /* [S] uniques per sample (length of dadaF$map / dadaR$map)                      */
+  const int32_t *dmapF, *dmapR;           /* [sum nuniq] dada maps (unique -> cluster), concatenated                       */
+  const int32_t *nclustF, *nclustR;       /* [S] clusters per sample                                                       */
+  const int32_t *n0F, *n0R;               /* [sum nclust] clustering$n0, concatenated                                      */
+  const char *seqF, *seqR;                /* cluster sequences, concatenated sample by sample ...                           */
+  const int64_t *seqF_off, *seqR_off;     /* ... [sum nclust + 1] offsets each                                             */
+} dada2b_pairs_in;
+
+typedef struct {
+  dada2b_merge_opts align;                /* scores, homo gap, trim_overhang; band must be -1                              */
+  int32_t min_overlap, max_mismatch;      /* accept = nmatch >= min_overlap && nmismatch + nindel <= max_mismatch          */
+  int32_t just_concatenate;               /* F + "NNNNNNNNNN" + rc(R); counts 0, prefer 0 (NA), accept 1, nothing aligned   */
+} dada2b_pairs_opts;
+
+typedef struct {
+  int32_t nsamples;
+  int64_t *pair_off;                      /* [S + 1] pairing offsets per sample                                            */
+  int32_t *forward, *reverse, *abundance; /* per pairing, 1-based cluster indices within the sample and read count          */
+  int32_t *nmatch, *nmismatch, *nindel, *prefer;
+  uint8_t *accept;
+  char *cons_concat;                      /* merged sequences, "" where rejected, concatenated ...                          */
+  int64_t *cons_off;                      /* ... [npairings + 1]                                                            */
+  /* work counters and timings (information only) */
+  int64_t n_reads, n_pairings, n_aligned, n_batches, n_cells, gpu_launches, h2d_bytes, d2h_bytes;
+  double ms_k_tab, ms_k_merge, ms_total;
+} dada2b_pairs_out;
+
+/* Samples are processed in batches of whole samples of at most DADA2B_PAIRS_BATCH reads (default 2^25; a larger sample runs
+ * alone); the distinct alignments of all batches run in one launch at the end.  Returns 0 on success, non-zero with a
+ * message in errbuf ("Non-corresponding derep-class and dada-class objects." as R/paired.R:116-119). */
+int dada2b_merge_samples(const dada2b_pairs_in *in, const dada2b_pairs_opts *opts, int32_t device, dada2b_pairs_out **out,
+                         char errbuf[DADA2B_ERRLEN]);
+void dada2b_merge_samples_free(dada2b_pairs_out *out);
+
 #ifdef __cplusplus
 }
 #endif
