@@ -3,6 +3,7 @@ reference's dada_uniques() interface.  See DESIGN.md / INTEGRATION.md."""
 from . import api  # noqa: F401
 from .api import Dada2bError, PackedCall, Resident, dada_uniques  # noqa: F401
 from . import bimera  # noqa: F401,E402
+from .bimera import removeBimeraDenovo  # noqa: F401,E402
 from . import merge  # noqa: F401,E402
 from . import derep  # noqa: F401,E402
 from . import errmodel  # noqa: F401,E402

@@ -3,6 +3,7 @@
 // Replaces (under /root/reference/src)
 //   C_table_bimera2 / BimeraTableParallel   chimera.cpp:61-207     -> dada2b_table_bimera
 //   C_is_bimera                             chimera.cpp:18-59      -> dada2b_is_bimera (batched)
+//   isBimeraDenovo's loop, every table row  R/chimeras.R:124-133   -> dada2b_denovo_bimera
 //   get_lr, get_ham_endsfree                chimera.cpp:210-269    -> bim_scan (on the traceback's 2-bit move string)
 // The alignment is the reference's nwalign_vectorized2(query, parent, match, mismatch, gap_p, end_gap 0, band max_shift)
 // (chimera.cpp:27, :122): the warp-per-pair banded ends-free NW of dd_nw_warp.cuh (bit-exact alignments, same kernel
@@ -15,6 +16,8 @@
 //                 -> one packed 64-bit record per (j, k)
 //   k_bim_flag    CTA per query, warp per sample: max of left / right (+ one-off variants) over the parents eligible
 //                 in that sample (coalesced reads of the sample-major count table and of the record row) -> nflag, nsam
+// The de novo call runs the same pipeline with isBimeraDenovo's parent rule in k_bim_need and k_bim_denovo_flag in
+// place of k_bim_flag: it counts the parents next to the maxima and writes one flag per (sample, query) cell.
 // Integer work throughout; no tensor cores by construction.  There is NO CPU fallback.
 #include "../../include/dada2b_bimera.h"
 #include "dd_common.h"
@@ -116,14 +119,29 @@ struct BimTableArgs {
   uint32_t j0; int jb;                      // queries [j0, j0 + jb) of this batch ...
   int q_mul, q_add;                         // ... query of batch slot s is (j0 + s) * q_mul + q_add (sharded calls own every world-th sequence)
   double min_fold; int min_abund, allow_one_off;
+  double min_parent_abund; int zero_queries;   // de novo rule only
   uint32_t *jq, *jk; unsigned long long *ctr;
   unsigned long long *rec;                  // [jb][ncol]
-  int32_t *nflag, *nsam;
+  int32_t *nflag, *nsam;                    // table call
+  uint8_t *flags;                           // de novo call: [ncol][nrow]
   const uint16_t *len;                      // [ncol] sequence lengths
 };
 
-// chimera.cpp:116-123: k is compared with j iff some sample i has mat(i,j) > 0, mat(i,k) > min_fold * mat(i,j) and
-// mat(i,k) >= min_abund.  grid (ceil(ncol / 256), jb); thread per candidate k, the query's column is read uniformly.
+// The two parent rules.  TABLE (C_table_bimera2, chimera.cpp:117-122): samples with mat(i,j) > 0, parents
+// mat(i,k) > min_fold * mat(i,j) and mat(i,k) >= min_abund.  DENOVO (isBimeraDenovo, R/chimeras.R:127): every sample
+// (zero-count queries too when zero_queries is set), parents strictly above a numeric minParentAbundance.
+enum BimRule { BIM_TABLE, BIM_DENOVO };
+template <BimRule RULE> __device__ __forceinline__ bool bim_query_in(const BimTableArgs &a, int vj) {
+  return RULE == BIM_DENOVO ? (vj > 0 || a.zero_queries) : vj > 0;
+}
+template <BimRule RULE> __device__ __forceinline__ bool bim_parent(const BimTableArgs &a, double bound, int vk) {
+  return RULE == BIM_DENOVO ? (double)vk > bound && (double)vk > a.min_parent_abund : (double)vk > bound && vk >= a.min_abund;
+}
+
+// k is compared with j iff k is a parent of j in some sample that takes j as a query (chimera.cpp:121-123: the reference
+// aligns a pair the first time a sample needs it).  grid (ceil(ncol / 256), jb); thread per candidate k, the query's
+// column is read uniformly.
+template <BimRule RULE>
 __global__ void __launch_bounds__(256) k_bim_need(BimTableArgs a) {
   const uint32_t slot = blockIdx.y;
   const uint32_t j = (a.j0 + slot) * (uint32_t)a.q_mul + (uint32_t)a.q_add;
@@ -134,9 +152,9 @@ __global__ void __launch_bounds__(256) k_bim_need(BimTableArgs a) {
     const int32_t *cj = a.mat + (size_t)j * a.nrow;
     for (int i = 0; i < a.nrow; i++) {
       const int vj = cj[i];
-      if (vj <= 0) continue;
+      if (!bim_query_in<RULE>(a, vj)) continue;
       const int vk = a.matT[(size_t)i * a.ncol + k];
-      if ((double)vk > a.min_fold * (double)vj && vk >= a.min_abund) { need = true; break; }
+      if (bim_parent<RULE>(a, a.min_fold * (double)vj, vk)) { need = true; break; }
     }
   }
   const unsigned m = __ballot_sync(0xffffffffu, need);
@@ -192,6 +210,50 @@ __global__ void __launch_bounds__(256) k_bim_flag(BimTableArgs a) {
   if (lane == 0) { if (nflag) atomicAdd(&s_flag, nflag); if (nsam) atomicAdd(&s_sam, nsam); }
   __syncthreads();
   if (threadIdx.x == 0) { a.nflag[j] = s_flag; a.nsam[j] = s_sam; }    // :172-173
+}
+
+// isBimeraDenovo's loop body (R/chimeras.R:124-132 + C_is_bimera, chimera.cpp:18-59) for every sample of one query, in
+// the shape of k_bim_flag: CTA per query, warp per sample.  The parents are counted with a ballot next to the six maxima;
+// fewer than two parents is FALSE without a model (:128-129).  Every cell (i, j) of the batch is written, 0 when the
+// sample does not take j as a query.
+__global__ void __launch_bounds__(256) k_bim_denovo_flag(BimTableArgs a) {
+  const uint32_t slot = blockIdx.x;
+  const uint32_t j = (a.j0 + slot) * (uint32_t)a.q_mul + (uint32_t)a.q_add;
+  const int nwarps = blockDim.x >> 5, wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int32_t *cj = a.mat + (size_t)j * a.nrow;
+  const unsigned long long *rrow = a.rec + (size_t)slot * a.ncol;
+  const int L = a.len[j];
+  for (int i = wid; i < a.nrow; i += nwarps) {
+    const int vj = cj[i];
+    bool bim = false;
+    if (bim_query_in<BIM_DENOVO>(a, vj)) {
+      const double bound = a.min_fold * (double)vj;
+      int npar = 0, ml = 0, mr = 0, ol = 0, orr = 0, olo = 0, oro = 0;
+      const int32_t *ti = a.matT + (size_t)i * a.ncol;
+      for (int k0 = 0; k0 < a.ncol; k0 += 32) {                         // warp-uniform trip count: the ballot sees every lane
+        const int k = k0 + lane;
+        const bool par = k < a.ncol && bim_parent<BIM_DENOVO>(a, bound, ti[k]);     // :127
+        npar += __popc(__ballot_sync(0xffffffffu, par));
+        if (par) {
+          const unsigned long long r = rrow[k];
+          const int l = (int)(r & 0x7FFF), rr = (int)((r >> 15) & 0x7FFF);
+          ml = max(ml, l); mr = max(mr, rr);                            // chimera.cpp:33-34
+          if (a.allow_one_off && (r & BIM_ALLOWED)) {                   // :37-42
+            ol = max(ol, l); orr = max(orr, rr);
+            olo = max(olo, (int)((r >> 30) & 0x7FFF)); oro = max(oro, (int)((r >> 45) & 0x7FFF));
+          }
+        }
+      }
+#pragma unroll
+      for (int o = 16; o; o >>= 1) {
+        ml = max(ml, __shfl_xor_sync(0xffffffffu, ml, o)); mr = max(mr, __shfl_xor_sync(0xffffffffu, mr, o));
+        ol = max(ol, __shfl_xor_sync(0xffffffffu, ol, o)); orr = max(orr, __shfl_xor_sync(0xffffffffu, orr, o));
+        olo = max(olo, __shfl_xor_sync(0xffffffffu, olo, o)); oro = max(oro, __shfl_xor_sync(0xffffffffu, oro, o));
+      }
+      bim = npar >= 2 && (mr + ml >= L || (a.allow_one_off && (ol + oro >= L || olo + orr >= L)));   // :45-52
+    }
+    if (lane == 0) a.flags[(size_t)j * a.nrow + i] = bim ? 1 : 0;
+  }
 }
 
 // C_is_bimera (chimera.cpp:18-59) for a batch: warp per query over its job range.
@@ -429,7 +491,7 @@ int dada2b_table_bimera(int32_t nrow, int32_t ncol, const int32_t *mat, const ch
       const int jb = (int)std::min<long long>(JB, nq - s0);
       ta.j0 = (uint32_t)s0; ta.jb = jb; R.aa.j0 = (uint32_t)s0;
       BCK(cudaMemsetAsync(R.d_rec.p, 0, (size_t)jb * ncol * 8, R.s));
-      k_bim_need<<<dim3((ncol + 255) / 256, jb), 256, 0, R.s>>>(ta);
+      k_bim_need<BIM_TABLE><<<dim3((ncol + 255) / 256, jb), 256, 0, R.s>>>(ta);
       R.launch_align((unsigned long long)jb * ncol);
       k_bim_flag<<<jb, 256, 0, R.s>>>(ta);
       k_bim_count<<<1, 1, 0, R.s>>>(ta.ctr);
@@ -438,6 +500,64 @@ int dada2b_table_bimera(int32_t nrow, int32_t ncol, const int32_t *mat, const ch
     BCK(cudaMemcpyAsync(nflag, d_nflag.p, (size_t)ncol * 4, cudaMemcpyDeviceToHost, R.s));
     BCK(cudaMemcpyAsync(nsam, d_nsam.p, (size_t)ncol * 4, cudaMemcpyDeviceToHost, R.s));
     R.d2h += (long long)ncol * 8;
+    R.finish(stats, t0);
+    return 0;
+  } catch (BErr &e) { return fail(errbuf, e.msg); }
+  catch (std::exception &e) { return fail(errbuf, e.what()); }
+}
+
+int dada2b_denovo_bimera(int32_t nrow, int32_t ncol, const int32_t *mat, const char *seq_concat, const int64_t *seq_off,
+                         const dada2b_bimera_opts *opts, double min_parent_abund, int32_t zero_queries, int32_t device,
+                         uint8_t *flags, dada2b_bimera_stats *stats, char errbuf[DADA2B_ERRLEN]) {
+  const double t0 = bnow_ms();
+  try {
+    check_opts(opts);
+    if (nrow < 0 || ncol <= 0) throw BErr{"Zero input sequences."};
+    if (opts->shard_world > 1 || opts->shard_rank != 0) throw BErr{"dada2b: the de novo bimera call is not sharded (shard_world must be 1)."};
+    if (min_parent_abund != min_parent_abund || opts->min_fold != opts->min_fold) throw BErr{"dada2b: NaN parent rule."};
+    const size_t cells = (size_t)nrow * ncol;
+    for (size_t c = 0; c < cells; c++)
+      if (mat[c] < 0) throw BErr{"dada2b: negative counts in the de novo bimera input."};
+    BimRun R;
+    R.open(device);
+    R.upload_seqs(ncol, seq_concat, seq_off);
+    R.setup_align(*opts);
+    BBuf<int32_t> d_mat, d_matT;
+    BBuf<uint8_t> d_flags;
+    d_mat.alloc(std::max<size_t>(cells, 1)); d_matT.alloc(std::max<size_t>(cells, 1)); d_flags.alloc(std::max<size_t>(cells, 1));
+    if (cells) {
+      BCK(cudaMemcpyAsync(d_mat.p, mat, cells * 4, cudaMemcpyHostToDevice, R.s));
+      R.h2d += (long long)cells * 4;
+      const int32_t *src = d_mat.p; int32_t *dst = d_matT.p;
+      k_bim_transpose<<<dim3((nrow + 31) / 32, (ncol + 31) / 32), dim3(32, 8), 0, R.s>>>(src, dst, nrow, ncol);
+      R.launches++;
+    }
+    // batch size as in the table call; DADA2B_BIM_JB=<n> caps it (test hook: small tables cross batch boundaries)
+    long long JB = std::min<long long>(65535, std::max<long long>(1, (2LL << 30) / (16LL * ncol)));
+    if (const char *e = getenv("DADA2B_BIM_JB")) { const long long cap = atoll(e); if (cap > 0) JB = std::min(JB, cap); }
+    JB = std::min<long long>(JB, ncol);
+    R.d_rec.alloc((size_t)JB * ncol); R.d_jq.alloc((size_t)JB * ncol); R.d_jk.alloc((size_t)JB * ncol);
+    BimTableArgs ta{};
+    ta.mat = d_mat.p; ta.matT = d_matT.p; ta.nrow = nrow; ta.ncol = ncol; ta.q_mul = 1; ta.q_add = 0;
+    ta.min_fold = opts->min_fold; ta.allow_one_off = opts->allow_one_off != 0;
+    ta.min_parent_abund = min_parent_abund; ta.zero_queries = zero_queries != 0;
+    ta.jq = R.d_jq.p; ta.jk = R.d_jk.p; ta.ctr = R.d_ctr.p; ta.rec = R.d_rec.p; ta.flags = d_flags.p; ta.len = R.d_len.p;
+    R.aa.jq = R.d_jq.p; R.aa.jk = R.d_jk.p; R.aa.njobs_ptr = R.d_ctr.p; R.aa.dst_mode = 1; R.aa.ncol = ncol; R.aa.rec = R.d_rec.p; R.aa.raw5 = nullptr;
+    R.aa.q_mul = 1; R.aa.q_add = 0;
+    for (long long s0 = 0; s0 < ncol && nrow > 0; s0 += JB) {
+      const int jb = (int)std::min<long long>(JB, ncol - s0);
+      ta.j0 = (uint32_t)s0; ta.jb = jb; R.aa.j0 = (uint32_t)s0;
+      BCK(cudaMemsetAsync(R.d_rec.p, 0, (size_t)jb * ncol * 8, R.s));
+      k_bim_need<BIM_DENOVO><<<dim3((ncol + 255) / 256, jb), 256, 0, R.s>>>(ta);
+      R.launch_align((unsigned long long)jb * ncol);
+      k_bim_denovo_flag<<<jb, 256, 0, R.s>>>(ta);
+      k_bim_count<<<1, 1, 0, R.s>>>(ta.ctr);
+      R.launches += 3;
+    }
+    if (cells) {
+      BCK(cudaMemcpyAsync(flags, d_flags.p, cells, cudaMemcpyDeviceToHost, R.s));
+      R.d2h += (long long)cells;
+    }
     R.finish(stats, t0);
     return 0;
   } catch (BErr &e) { return fail(errbuf, e.msg); }

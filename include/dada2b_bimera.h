@@ -68,6 +68,18 @@ int dada2b_is_bimera(int32_t nseq, const char *seq_concat, const int64_t *seq_of
                      const dada2b_bimera_opts *opts, int32_t device, uint8_t *is_bimera, dada2b_bimera_stats *stats,
                      char errbuf[DADA2B_ERRLEN]);
 
+/* isBimeraDenovo (R/chimeras.R:124-133) applied to every row of a table: flags(i,j) = 1 iff
+ *   (mat(i,j) > 0 || zero_queries) and |P(i,j)| >= 2 and C_is_bimera(seq j, P(i,j)),
+ *   P(i,j) = { k : (double)mat(i,k) > min_fold * (double)mat(i,j)  &&  (double)mat(i,k) > min_parent_abund }.
+ * mat / flags: column-major nrow x ncol as in dada2b_table_bimera; flags caller-allocated uint8[nrow*ncol].
+ * A one-row call with zero_queries = 1 is isBimeraDenovo on a uniques vector (R evaluates zero abundances too); a
+ * per-sample table passes zero_queries = 0, because a flagged zero cell stays zero.  Each (j, k) pair is aligned at most
+ * once across all rows.  opts->min_abund is not used; opts->shard_world must be 1.  Negative counts are rejected.
+ * stats may be NULL. */
+int dada2b_denovo_bimera(int32_t nrow, int32_t ncol, const int32_t *mat, const char *seq_concat, const int64_t *seq_off,
+                         const dada2b_bimera_opts *opts, double min_parent_abund, int32_t zero_queries, int32_t device,
+                         uint8_t *flags, dada2b_bimera_stats *stats, char errbuf[DADA2B_ERRLEN]);
+
 /* Kernel-level hook for the parity tests: align each (query, parent) pair and return what chimera.cpp's get_lr
  * (:239-269) and get_ham_endsfree (:210-236) compute on the alignment.  out5: int32[npairs][5] =
  * {left, right, left_oo, right_oo, ham}; left_oo / right_oo are only defined when allow_one_off is set. */
