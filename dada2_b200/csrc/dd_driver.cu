@@ -227,6 +227,7 @@ struct dada2b_ctx {
   DBuf<uint8_t> d_qual_own, d_seq_own, d_seq_all;
   DBuf<int> d_flags;
   unsigned total_reads = 0;
+  int reads_argmax = -1;          // first raw with the largest abundance (bi_assign_center of the initial cluster), -1 if all are 0
   std::vector<uint16_t> len;
   std::vector<uint32_t> reads;
   std::vector<uint8_t> prior;
@@ -368,7 +369,8 @@ static dada2b_ctx *do_upload(const dada2b_in *in, int device, dada2b_ctx *reuse 
     }
     cudaError_t copy_err = cudaSuccess;
     {  // meanwhile: abundances / priors / lengths (7 bytes per raw) from the calling thread
-      unsigned tot = 0;
+      unsigned tot = 0, mx = 0;
+      int amax = -1;
       uint8_t *m = cx->st_meta.p;
       uint32_t *m_reads = (uint32_t *)m; uint8_t *m_prior = m + (size_t)nraw * 6;
       for (unsigned i = 0; i < nraw; i++) {
@@ -376,8 +378,9 @@ static dada2b_ctx *do_upload(const dada2b_in *in, int device, dada2b_ctx *reuse 
         const uint8_t pr = in->prior ? (in->prior[i] != 0) : 0;
         cx->reads[i] = rd; cx->prior[i] = pr; m_reads[i] = rd; m_prior[i] = pr;
         tot += rd;                                              // unsigned int accumulation, containers.cpp:100
+        if (rd > mx) { mx = rd; amax = (int)i; }
       }
-      cx->total_reads = tot;
+      cx->total_reads = tot; cx->reads_argmax = amax;
       memcpy(m + (size_t)nraw * 4, cx->len.data(), (size_t)nraw * 2);
       copy_err = cudaMemcpyAsync(cx->d_reads.p, m, (size_t)nraw * 4, cudaMemcpyHostToDevice, cx->stream);
       if (copy_err == cudaSuccess) copy_err = cudaMemcpyAsync(cx->d_len.p, m + (size_t)nraw * 4, (size_t)nraw * 2, cudaMemcpyHostToDevice, cx->stream);
@@ -442,10 +445,11 @@ dada2b_ctx *ctx_create_device(int device, int nraw, int maxlen, int minlen, cons
     CK(cudaStreamCreateWithFlags(&cx->stream, cudaStreamNonBlocking));
     cx->has_quals = true; cx->bad_nt = false; cx->maxq = 0;
     cx->len.resize(nraw); cx->reads.resize(nraw); cx->prior.assign(nraw, 0);
-    unsigned tot = 0;
+    unsigned tot = 0, mx = 0;
     for (int i = 0; i < nraw; i++) {
       cx->len[i] = (uint16_t)(seq_off[i + 1] - seq_off[i]);
       cx->reads[i] = (uint32_t)abund[i]; tot += cx->reads[i];
+      if (cx->reads[i] > mx) { mx = cx->reads[i]; cx->reads_argmax = i; }
     }
     cx->total_reads = tot;
     DevIn &d = cx->in;
@@ -521,7 +525,9 @@ struct Run {
   // scratch of the rare paths and of finish(): members, so that a steady-state pass makes no cudaMalloc / cudaFree (those go through the
   // kernel driver and wait behind whatever else holds its lock, e.g. a monitoring agent polling the GPU)
   DBuf<uint32_t> tie_d1, tie_d2, tie_g1, tie_g2, fin_nwl, fin_gll, fin_sij, fin_gij;
-  DBuf<unsigned long long> win_buf, fin_dcount, fin_dall;
+  DBuf<unsigned long long> win_buf, fin_dcount, fin_dall, fin_keep;
+  DBuf<uint32_t> fin_tl;                // per-cluster tallies of finish(): abundance, n0, n1, nunq, largest member reads (dd_final.cu)
+  DBuf<int32_t> fin_map;
   DBuf<uint8_t> fin_cq, fin_rep_d;
   DBuf<uint32_t> fin_rep_rows;
   DBuf<uint32_t> ft_off, ft_chk, ft_cur, ft_ord, ft_sums;   // k_final_tally's per-cluster offsets and cluster-ordered raws (dd_final.cu)
@@ -563,7 +569,7 @@ struct Run {
   int nclust_h = 0;
   // b_shuffle2's container updates and b_bud's pop / new cluster are pure host bookkeeping (O(moves), but ~30 ms of a 1e6-unique
   // run): the device reports everything the next bud decision needs unless it is an exact tie, so the updates
-  // are queued to a worker and applied while the GPU runs the next round.
+  // are queued to a worker and applied while the GPU runs the next round.  kind: 0 moves, 1 bud, 2 cluster 0's member arrays.
   struct ReplayEvent { int kind; std::vector<uint32_t> mv; std::vector<uint32_t> pass_end; uint32_t r, from, ni; };
   bool async_replay = false;
   std::thread rworker;
@@ -573,6 +579,7 @@ struct Run {
   bool rbusy = false, rquit = false;
   void apply_moves(const uint32_t *mv, size_t n);
   void apply_bud(uint32_t r, uint32_t from);
+  void init_members();
   void push_event(ReplayEvent &&e);
   void drain_replay();
   void stop_replay();
@@ -785,6 +792,7 @@ void Run::alloc_state() {
     }
   } else { row_mv.free(); row_sub.free(); lane_max = 0; }
   prescreen = P.use_kmers && !fallback_only;
+  bool read_novf = false;
   if (prescreen) {
     nown = (nraw - scr_rank + scr_world - 1) / scr_world;
     kbits.alloc((size_t)nown * 32 + 32); kmeta.alloc(nown); krep.alloc((size_t)nown * 48 + 64); cand_list.alloc(nown + 32); cand_ms.alloc(nown + 32);
@@ -792,8 +800,9 @@ void Run::alloc_state() {
     if (kbits_gen != cx->upload_gen) {       // the bitmaps and repeat lists depend on the sequences only: kept across the runs of a resident sample
       d_novf.alloc(1); d_novf.zero(s);
       launch_kmer_bits(in, scr_rank, scr_world, nown, kbits.p, kmeta.p, krep.p, d_novf.p, scr_sms, s);
-      d2h(&n_ovf, d_novf.p, 4);            // read by the sync() at the end of alloc_state
+      d2h(&n_ovf, d_novf.p, 4);            // launch_screen reads it: synchronised below
       kbits_gen = cx->upload_gen;
+      read_novf = true;
     }
   }
   if (const char *e = getenv("DADA2B_NP")) NP = std::max(1, std::min(MAX_PASS, atoi(e)));      // tuning / test override
@@ -822,8 +831,7 @@ void Run::alloc_state() {
   cluster_of.zero(s); ctr.zero(s);
   launch_fill_f64(E_minmax.p, -999.0, n, s);                      // containers.cpp:39
   TDBG("alloc: memsets queued");
-  sync();
-  TDBG("alloc: synced");
+  if (read_novf) sync();
   st.lock = lock.p; st.is_center = is_center.p; st.slot0 = slot0.p; st.correct = correct.p;
   st.E_minmax = E_minmax.p; st.p = p.p; st.comp_lambda = comp_lambda.p; st.comp_ham = comp_ham.p; st.cluster_of = cluster_of.p;
   st.nw_list = nw_list.p; st.gl_list = gl_list.p;
@@ -832,7 +840,6 @@ void Run::alloc_state() {
   st.shard_rank = cx->rank; st.shard_world = cx->world;
   st.report = (RoundReport *)d_repmv.p; st.moves = (uint32_t *)(d_repmv.p + RR_PAD);
   { unsigned long long nn = n; h2d(ctr.p + CTR_CS_COUNT, &nn, 8); }  // cluster 0 owns entries [0, nraw)
-  sync();
   st.cs_cap = 0;
   ensure_cs_cap(2ull * n + 1024);
   TDBG("alloc: cs cap");
@@ -840,7 +847,6 @@ void Run::alloc_state() {
   st.cl_reads = cl_reads.p; st.cl_center = cl_center.p;
   st.cl_update_e = cl_update_e.p; st.cl_check_locks = cl_check_locks.p;
   cl_reads.zero(s); cl_center.zero(s); cl_update_e.zero(s); cl_check_locks.zero(s);
-  sync();
   TDBG("alloc: cluster cap");
   if (!ptr_in_smem) {
     ptr_scratch.alloc((size_t)ptr_words * align_grid * 4);
@@ -1146,6 +1152,13 @@ void Run::apply_bud(uint32_t r, uint32_t from) {
   cl_reads_h.push_back(cx->reads[r]);
 }
 
+// b_init (containers.cpp:78-137): every raw in cluster 0, slot = index
+void Run::init_members() {
+  members.assign(1, std::vector<uint32_t>(nraw));
+  slot_of.resize(nraw); cluster_of_h.assign(nraw, 0);
+  for (int r = 0; r < nraw; r++) { members[0][r] = r; slot_of[r] = r; }
+}
+
 void Run::push_event(ReplayEvent &&e) {
   std::unique_lock<std::mutex> lk(rmu);
   if (!rworker.joinable()) {
@@ -1162,7 +1175,8 @@ void Run::push_event(ReplayEvent &&e) {
         if (ev.kind == 0) {
           size_t b = 0;
           for (uint32_t e2 : ev.pass_end) { apply_moves(ev.mv.data() + 2 * b, e2 - b); b = e2; }
-        } else apply_bud(ev.r, ev.from);
+        } else if (ev.kind == 1) apply_bud(ev.r, ev.from);
+        else init_members();
         lk2.lock();
         rbusy = false;
         if (rq.empty()) rdone.notify_all();
@@ -1305,8 +1319,17 @@ template <typename T> T *dupv(const std::vector<T> &v) {
 void Run::finish(dada2b_out *out) {
   // DADA2B_VERBOSE: host clock per phase; the device work of a phase is waited for before its end is read
   const bool vb = getenv("DADA2B_VERBOSE") != nullptr;
-  double ph[7]; int nph = 0;
+  double ph[10]; int nph = 0;
   ph[nph++] = now_ms();
+  // A helper sums the loop's kernel timings while the device runs the final pass (every event recorded so far has completed:
+  // the loop ended with a synchronisation); ~2.5 ms of event queries at 1e6 uniques.  The guard joins it on every way out.
+  const std::vector<Ev> loop_evs(evs);
+  double ksum[T_N] = {}; int kcnt[T_N] = {};
+  std::thread ev_helper([&]() {
+    if (cudaSetDevice(cx->device) != cudaSuccess) return;
+    for (const Ev &e : loop_evs) { float t = 0; if (cudaEventElapsedTime(&t, e.a, e.b) == cudaSuccess) { ksum[e.tag] += t; kcnt[e.tag]++; } }
+  });
+  struct Join { std::thread &t; ~Join() { if (t.joinable()) t.join(); } } join{ev_helper};
   drain_replay();
   ph[nph++] = now_ms();
   const uint32_t nclust = (uint32_t)members.size();
@@ -1317,7 +1340,6 @@ void Run::finish(dada2b_out *out) {
   cq_sum.alloc((size_t)nclust * maxlen); cq_cnt.alloc((size_t)nclust * maxlen); cq_sum.zero(s); cq_cnt.zero(s);
   st.trans = trans.p; st.cq_sum = cq_sum.p; st.cq_cnt = cq_cnt.p;
   const int n_owned = (nraw - cx->rank + cx->world - 1) / cx->world;     // raws aligned by this rank in the final pass
-  if (cx->world > 1) nsubs_final.zero(s);
   bool split = false;                    // the raws are split into a diagonal and a gapped list
   {  // FinalSubsParallel: sub_new(centre, raw, use_kmers=false) for every raw
     if (P.band > 0) {
@@ -1362,6 +1384,8 @@ void Run::finish(dada2b_out *out) {
       timed(T_FGAP, [&]() { launch_align_jobs(MODE_FINAL, a, (unsigned long long)nraw); });
     }
   }
+  fin_tl.alloc((size_t)5 * nclust); fin_tl.zero(s); fin_map.alloc(nraw);
+  launch_cluster_tally(in, st, (int)nclust, cx->rank, cx->world, fin_tl.p, fin_map.p, cx->num_sms, s);
   if (vb) {
     read_ctr();                            // synchronises
     if (split) fprintf(stderr, "[dada2b] final pass lists: diagonal %llu, gapped %llu, handed back %llu\n", h_ctr.p[CTR_GL], h_ctr.p[CTR_NW], h_ctr.p[CTR_NMOVE]);
@@ -1371,11 +1395,13 @@ void Run::finish(dada2b_out *out) {
     NC(g_nccl.AllReduce(trans.p, trans.p, (size_t)16 * ncol, ncclInt32, ncclSum, cx->comm, s));
     NC(g_nccl.AllReduce(cq_sum.p, cq_sum.p, (size_t)nclust * maxlen, ncclUint64, ncclSum, cx->comm, s));
     NC(g_nccl.AllReduce(cq_cnt.p, cq_cnt.p, (size_t)nclust * maxlen, ncclUint64, ncclSum, cx->comm, s));
-    NC(g_nccl.AllReduce(nsubs_final.p, nsubs_final.p, (size_t)nraw, ncclUint32, ncclSum, cx->comm, s));
-    // final p / correct are only meaningful on a raw's owner: zero the rest, then the sum is the full array
+    NC(g_nccl.AllReduce(fin_tl.p, fin_tl.p, (size_t)4 * nclust, ncclUint32, ncclSum, cx->comm, s));
+    // abundances arrive as non-negative int32: their int32 maximum is the unsigned one
+    NC(g_nccl.AllReduce(fin_tl.p + (size_t)4 * nclust, fin_tl.p + (size_t)4 * nclust, nclust, ncclInt32, ncclMax, cx->comm, s));
+    NC(g_nccl.AllReduce(fin_map.p, fin_map.p, (size_t)nraw, ncclInt32, ncclSum, cx->comm, s));     // 0 off the owner
+    // final p is only meaningful on a raw's owner: zero the rest, then the sum is the full array
     launch_mask_unowned(this->p.p, correct.p, nraw, cx->rank, cx->world, s);
     NC(g_nccl.AllReduce(this->p.p, this->p.p, (size_t)nraw, ncclFloat64, ncclSum, cx->comm, s));
-    NC(g_nccl.AllReduce(correct.p, correct.p, (size_t)nraw, ncclUint8, ncclSum, cx->comm, s));
   }
   // birth subs: sub_new(centre of birth_comp.i, centre i, use_kmers, cutoff 1.0)   Rmain.cpp:206-209
   const uint32_t npair = nclust - 1;
@@ -1403,9 +1429,10 @@ void Run::finish(dada2b_out *out) {
     ca.in = in; ca.P = P; ca.P.kdist_cutoff = 1.0; ca.mode = 1; ca.pair_centre = pair_centre.p; ca.pair_raw = pair_raw.p;
     ca.nw_list = nwl.p; ca.gl_list = gll.p; ca.ctr = st.ctr; ca.kord_words = kord_words; ca.greedy = 0; ca.lock = st.lock;
     ca.shard_rank = 0; ca.shard_world = 1;
-    // birth alignments are not counted in nalign/nshroud by the reference; restore the counters afterwards
-    read_ctr();
-    unsigned long long keepA = h_ctr.p[CTR_ALIGN], keepS = h_ctr.p[CTR_SHROUD];
+    // birth alignments are not counted in nalign/nshroud by the reference: the counters are kept on the device and restored afterwards
+    static_assert(CTR_SHROUD == CTR_ALIGN + 1, "counter layout");
+    DBuf<unsigned long long> &keep = fin_keep; keep.alloc(2);
+    CK(cudaMemcpyAsync(keep.p, ctr.p + CTR_ALIGN, 2 * 8, cudaMemcpyDeviceToDevice, s));
     launch_classify(ca, (int)npair, 256, classify_smem, s);
     for (int kind : {KIND_NW, KIND_GAPLESS}) {
       AlignArgs a = align_args(MODE_BIRTH, kind);
@@ -1416,15 +1443,13 @@ void Run::finish(dada2b_out *out) {
       a.b_cap = bcap; a.b_ops = nullptr; a.b_nops = nullptr; a.b_opcap = 0;
       launch_align_jobs(MODE_BIRTH, a, npair);
     }
-    h2d(ctr.p + CTR_ALIGN, &keepA, 8);
-    h2d(ctr.p + CTR_SHROUD, &keepS, 8);
+    CK(cudaMemcpyAsync(ctr.p + CTR_ALIGN, keep.p, 2 * 8, cudaMemcpyDeviceToDevice, s));
     bpos.resize((size_t)npair * bcap); bnt0.resize((size_t)npair * bcap); bnt1.resize((size_t)npair * bcap); bq1.resize((size_t)npair * bcap);
     d2h(bns.data(), b_nsubs.p, npair * 4);
     d2h(bpos.data(), b_pos.p, bpos.size() * 2);
     d2h(bnt0.data(), b_nt0.p, bnt0.size());
     d2h(bnt1.data(), b_nt1.p, bnt1.size());
-    d2h(bq1.data(), b_q1.p, bq1.size());
-    sync();
+    d2h(bq1.data(), b_q1.p, bq1.size());           // completed by the post-hoc pass's first synchronisation
   }
   ph[nph++] = now_ms();
   // post-hoc cluster p-values (error.cpp:99-119)
@@ -1494,17 +1519,20 @@ void Run::finish(dada2b_out *out) {
   }
   if (vb) sync();
   ph[nph++] = now_ms();
-  // per-raw results: staged in the pinned arena and written straight into the output arrays by several threads
+  // cluster-sized results, $map and $pval: staged in the pinned arena, one synchronisation for all of them
   std::vector<int> htrans((size_t)16 * ncol); std::vector<unsigned long long> hsum((size_t)nclust * maxlen), hcnt((size_t)nclust * maxlen);
+  std::vector<uint32_t> tl((size_t)5 * nclust);
+  {
+    const size_t need = htrans.size() * 4 + (hsum.size() + hcnt.size()) * 8 + tl.size() * 4 + (size_t)nraw * 12 + 6 * 64;
+    if (arena_off + need > arena.cap) { sync(); if (need > arena.cap) arena.alloc(need); }   // nothing staged below waits for room
+  }
   d2h(htrans.data(), trans.p, htrans.size() * 4);
   d2h(hsum.data(), cq_sum.p, hsum.size() * 8);
   d2h(hcnt.data(), cq_cnt.p, hcnt.size() * 8);
-  sync();                                         // the arena is empty from here on
-  if ((size_t)nraw * 13 + 256 > arena.cap) arena.alloc((size_t)nraw * 13 + 256);
+  d2h(tl.data(), fin_tl.p, tl.size() * 4);
   auto stage = [&](const void *d, size_t n) { d2h_bytes += (long long)n; uint8_t *q = arena_get(n); CK(cudaMemcpyAsync(q, d, n, cudaMemcpyDeviceToHost, s)); return q; };
   const double *hp = (const double *)stage(p.p, (size_t)nraw * 8);
-  const uint32_t *hns = (const uint32_t *)stage(nsubs_final.p, (size_t)nraw * 4);
-  const uint8_t *hcorrect = stage(correct.p, nraw);
+  const int32_t *hmap = (const int32_t *)stage(fin_map.p, (size_t)nraw * 4);
   read_ctr();                                     // synchronises; nothing below touches the arena
   check_dev_error();
   ph[nph++] = now_ms();
@@ -1515,27 +1543,12 @@ void Run::finish(dada2b_out *out) {
   out->n_rounds = n_rounds; out->n_shuffles = n_shuffles;
   // ---- $clustering (error.cpp:9-127)
   std::string cseq; std::vector<int64_t> coff(1, 0);
-  std::vector<int32_t> ab(nclust, 0), n0(nclust, 0), n1(nclust, 0), nunq(nclust, 0), bfrom(nclust), bham(nclust);
+  std::vector<int32_t> ab(nclust), n0(nclust), n1(nclust), nunq(nclust), bfrom(nclust), bham(nclust);
   std::vector<double> bpval(nclust), bfold(nclust), bqave(nclust);
-  std::vector<uint32_t> mxr(nclust, 0);            // largest abundance among a cluster's members (correct or not)
-  {
-    std::mutex mu;
-    parallel_for((size_t)nraw, [&](size_t lo, size_t hi) {       // integer tallies: order-independent
-      std::vector<int32_t> a(nclust, 0), z0(nclust, 0), z1(nclust, 0), nu(nclust, 0);
-      std::vector<uint32_t> mx(nclust, 0);
-      for (size_t r = lo; r < hi; r++) {
-        const uint32_t i = cluster_of_h[r], rd = cx->reads[r];
-        mx[i] = std::max(mx[i], rd);
-        if (hcorrect[r]) {
-          a[i] += (int32_t)rd; nu[i]++;
-          if (hns[r] == 0) z0[i] += (int32_t)rd;
-          if (hns[r] == 1) z1[i] += (int32_t)rd;
-        }
-      }
-      std::lock_guard<std::mutex> lk(mu);
-      for (uint32_t i = 0; i < nclust; i++) { ab[i] += a[i]; n0[i] += z0[i]; n1[i] += z1[i]; nunq[i] += nu[i]; mxr[i] = std::max(mxr[i], mx[i]); }
-    });
+  for (uint32_t i = 0; i < nclust; i++) {
+    ab[i] = (int32_t)tl[i]; n0[i] = (int32_t)tl[nclust + i]; n1[i] = (int32_t)tl[2 * (size_t)nclust + i]; nunq[i] = (int32_t)tl[3 * (size_t)nclust + i];
   }
+  const uint32_t *mxr = tl.data() + 4 * (size_t)nclust;    // largest abundance among a cluster's members (correct or not)
   // The representative sequences are read back from the packed rows on the device (a run that gets here saw nothing but ACGT,
   // nt2int would have stopped it): no host copy of the input strings is kept.  Pinned buffer of its own -- the arena is in use.
   std::vector<long> max_raw(nclust, -1);           // error.cpp:20-27: the first member (Bi::raw order) holding the largest abundance
@@ -1555,6 +1568,7 @@ void Run::finish(dada2b_out *out) {
     CK(cudaMemcpyAsync(fin_rep_h.p + (((size_t)nrep * 4 + 63) & ~(size_t)63), fin_rep_d.p, (size_t)nrep * rowb, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
   }
+  ph[nph++] = now_ms();
   const uint32_t *rep_words = (const uint32_t *)(fin_rep_h.p + (((size_t)nrep * 4 + 63) & ~(size_t)63));
   uint32_t rep_k = 0;
   for (uint32_t i = 0; i < nclust; i++) {
@@ -1602,21 +1616,28 @@ void Run::finish(dada2b_out *out) {
     }
   }
   out->clusterquals = dupv(cq);
+  ph[nph++] = now_ms();
   // ---- $map, $pval (Rmain.cpp:239-279)
   out->map = (int32_t *)malloc(std::max<size_t>(1, nraw) * sizeof(int32_t));
   out->pval = (double *)malloc(std::max<size_t>(1, nraw) * sizeof(double));
   parallel_for((size_t)nraw, [&](size_t lo, size_t hi) {
-    for (size_t r = lo; r < hi; r++) out->map[r] = hcorrect[r] ? (int32_t)cluster_of_h[r] + 1 : INT_MIN;
+    memcpy(out->map + lo, hmap + lo, (hi - lo) * sizeof(int32_t));
     memcpy(out->pval + lo, hp + lo, (hi - lo) * sizeof(double));
   });
+  ph[nph++] = now_ms();
   // ---- timing / traffic diagnostics
   CK(cudaEventRecord(ev_end, s));
   CK(cudaEventSynchronize(ev_end));
   float ms = 0;
   CK(cudaEventElapsedTime(&ms, ev_begin, ev_end));
   out->ms_device = ms;
+  ev_helper.join();
   double sum[T_N] = {}; int cnt[T_N] = {};
-  for (const Ev &e : evs) { float t = 0; if (cudaEventElapsedTime(&t, e.a, e.b) == cudaSuccess) { sum[e.tag] += t; cnt[e.tag]++; } }
+  for (int t = 0; t < T_N; t++) { sum[t] = ksum[t]; cnt[t] = kcnt[t]; }
+  for (size_t k = loop_evs.size(); k < evs.size(); k++) {        // the final pass's
+    const Ev &e = evs[k]; float t = 0;
+    if (cudaEventElapsedTime(&t, e.a, e.b) == cudaSuccess) { sum[e.tag] += t; cnt[e.tag]++; }
+  }
   if (getenv("DADA2B_VERBOSE")) fprintf(stderr, "[dada2b] loop NW: bound pass %.3f ms (%d launches), exact %.3f ms (%d launches)\n", sum[T_NWB], cnt[T_NWB], sum[T_NW], cnt[T_NW]);
   out->ms_k_prescreen = sum[T_PRE]; out->n_k_prescreen = cnt[T_PRE]; out->prescreen_rows = prescreen_rows;
   out->ms_k_nw_bound = sum[T_NWB]; out->n_k_nw_bound = cnt[T_NWB]; out->ms_k_nw_exact = sum[T_NW]; out->n_k_nw_exact = cnt[T_NW];
@@ -1631,8 +1652,9 @@ void Run::finish(dada2b_out *out) {
   out->gpu_launches = launches_count() - launches0;
   out->h2d_bytes = h2d_bytes; out->d2h_bytes = d2h_bytes;
   ph[nph++] = now_ms();
-  if (vb) fprintf(stderr, "[dada2b] finish host ms: drain replay %.2f, final pass %.2f, birth subs %.2f, post-hoc %.2f, D2H %.2f, host tallies/output %.2f\n",
-                  ph[1] - ph[0], ph[2] - ph[1], ph[3] - ph[2], ph[4] - ph[3], ph[5] - ph[4], ph[6] - ph[5]);
+  if (vb) fprintf(stderr, "[dada2b] finish host ms: drain replay %.2f, final pass %.2f, birth subs %.2f, post-hoc %.2f, D2H %.2f, "
+                  "representatives %.2f, cluster outputs %.2f, map/pval %.2f, kernel timings %.2f\n",
+                  ph[1] - ph[0], ph[2] - ph[1], ph[3] - ph[2], ph[4] - ph[3], ph[5] - ph[4], ph[6] - ph[5], ph[7] - ph[6], ph[8] - ph[7], ph[9] - ph[8]);
 }
 
 dada2b_out *do_run(dada2b_ctx *cx, const double *err_cm, int Q, const dada2b_opts *o) {
@@ -1663,18 +1685,12 @@ dada2b_out *do_run(dada2b_ctx *cx, const double *err_cm, int Q, const dada2b_opt
     for (int r = 0; r < 16; r++) for (int c = 0; c < Q; c++) e[(size_t)r * Q + c] = err_cm[r + 16 * (size_t)c];
     R.h2d(R.err.p, e.data(), e.size() * 8);
     if (R.two_phase) launch_raw_bounds(R.in, R.err.p, Q, o->use_quals != 0, R.raw_S.p, R.raw_rho.p, cx->rank, cx->world, R.s);
-    R.sync();
   }
-  const int nraw = R.nraw;
-  // b_new / b_init (containers.cpp:78-137): one cluster holding every raw in index order
-  R.members.emplace_back(nraw);
+  // b_new / b_init (containers.cpp:78-137): one cluster holding every raw in index order; its centre is the first raw with the
+  // largest abundance (bi_assign_center), found when the abundances were uploaded
+  if (cx->reads_argmax < 0) throw Err{"dada2b: all abundances are zero."};
+  const uint32_t c0 = (uint32_t)cx->reads_argmax;
   R.nclust_h = 1;
-  for (int r = 0; r < nraw; r++) R.members[0][r] = r;
-  R.slot_of.resize(nraw); R.cluster_of_h.assign(nraw, 0);
-  for (int r = 0; r < nraw; r++) R.slot_of[r] = r;
-  uint32_t c0 = 0, mx = 0; bool found = false;
-  for (int r = 0; r < nraw; r++) if (cx->reads[r] > mx) { mx = cx->reads[r]; c0 = r; found = true; }   // bi_assign_center
-  if (!found) throw Err{"dada2b: all abundances are zero."};
   R.cl_center_h.push_back(c0); R.cl_reads_h.push_back(cx->total_reads);
   R.birth.emplace_back(); R.birth[0].e = cx->total_reads;
   {
@@ -1684,11 +1700,13 @@ dada2b_out *do_run(dada2b_ctx *cx, const double *err_cm, int Q, const dada2b_opt
     R.h2d(R.cl_reads.p, &cx->total_reads, 4);
     R.h2d(R.cl_center.p, &c0, 4);
     R.h2d(R.cl_update_e.p, &one, 1); R.h2d(R.cl_check_locks.p, &one, 1);
-    R.sync();
   }
   // host bookkeeping off the critical path (see Run::ReplayEvent): needs every cluster's centre at slot 0 (abundance-sorted input,
-  // what derepFastq produces); DADA2B_SYNC_REPLAY is a test hook
+  // what derepFastq produces); DADA2B_SYNC_REPLAY is a test hook.  The member arrays of cluster 0 are then filled by the replay
+  // worker while round 0 runs: they are first read by a replayed event or after drain_replay().
   R.async_replay = c0 == 0 && getenv("DADA2B_SYNC_REPLAY") == nullptr;
+  if (R.async_replay) R.push_event(Run::ReplayEvent{2, {}, {}, 0, 0, 0});
+  else R.init_members();
   TDBG("cluster 0 initialised");
   const double t1 = now_ms();
   const bool dbg = o->verbose || getenv("DADA2B_VERBOSE");
@@ -1697,7 +1715,7 @@ dada2b_out *do_run(dada2b_ctx *cx, const double *err_cm, int Q, const dada2b_opt
   R.launch_round_tail(0, 0);                 // initial cluster: b_p_update + first b_bud scan
   R.sync_report();
   if (dbg) fprintf(stderr, "[dada2b] round 0 done: %.2f ms, cs=%llu\n", now_ms() - t1, R.cs_count);
-  const int max_clust = o->max_clust < 1 ? nraw : o->max_clust;
+  const int max_clust = o->max_clust < 1 ? R.nraw : o->max_clust;
   uint32_t wr = 0, wfrom = 0;
   int newi;
   double h_enq = 0, h_wait = 0, h_replay = 0, h_decide = 0;      // host time per phase of a round (verbose diagnostics)

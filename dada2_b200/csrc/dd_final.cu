@@ -163,7 +163,48 @@ __global__ void __launch_bounds__(FT_THREADS) k_final_tally(FtArgs a) {
     if (s_trans[x]) atomicAdd(&a.st.trans[x], s_trans[x]);
 }
 
+__device__ __forceinline__ void ct_add(uint32_t *t, size_t stride, uint32_t rd, bool ok, uint32_t ns) {
+  atomicMax(&t[4 * stride], rd);
+  if (!ok) return;
+  atomicAdd(&t[0], rd);
+  atomicAdd(&t[3 * stride], 1u);
+  if (ns == 0) atomicAdd(&t[stride], rd);
+  else if (ns == 1) atomicAdd(&t[2 * stride], rd);
+}
+
+// One thread per raw of this rank (raw r with r % world == rank): the per-cluster tallies of $clustering (error.cpp:9-52) and
+// $map (Rmain.cpp:239-279).  tl = [abundance | n0 | n1 | nunq | largest reads of any member] x nclust, zeroed by the caller.
+// map[r] = cluster + 1 where correct, INT_MIN where not, 0 for the other ranks' raws (a sum all-reduce completes it).
+// Sums wrap modulo 2^32 like the int32 sums they restate; every result is an integer sum or maximum, so order-independent.
+__global__ void __launch_bounds__(FT_THREADS) k_cluster_tally(DevIn in, DevState st, int nclust, int rank, int world, uint32_t *tl, int32_t *map) {
+  __shared__ uint32_t s_tl[5 * FT_SMEM_CL];
+  const uint32_t H = (uint32_t)min(nclust, FT_SMEM_CL);
+  for (int x = threadIdx.x; x < 5 * FT_SMEM_CL; x += blockDim.x) s_tl[x] = 0;
+  __syncthreads();
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < in.nraw; r += gridDim.x * blockDim.x) {
+    if (r % world != rank) { map[r] = 0; continue; }
+    const uint32_t cl = st.cluster_of[r], rd = in.reads[r], ns = st.nsubs_final[r];
+    const bool ok = st.correct[r] != 0;
+    map[r] = ok ? (int32_t)cl + 1 : INT_MIN;
+    if (cl < H) ct_add(&s_tl[cl], FT_SMEM_CL, rd, ok, ns);
+    else ct_add(&tl[cl], (size_t)nclust, rd, ok, ns);
+  }
+  __syncthreads();
+  for (uint32_t x = threadIdx.x; x < 5 * H; x += blockDim.x) {
+    const uint32_t k = x / H, cl = x % H, v = s_tl[k * FT_SMEM_CL + cl];
+    if (!v) continue;
+    if (k == 4) atomicMax(&tl[4 * (size_t)nclust + cl], v);
+    else atomicAdd(&tl[k * (size_t)nclust + cl], v);
+  }
+}
+
 }  // namespace
+
+void launch_cluster_tally(const DevIn &in, const DevState &st, int nclust, int rank, int world, uint32_t *tl, int32_t *map, int num_sms, cudaStream_t s) {
+  const int grid = std::max(1, std::min((in.nraw + FT_THREADS - 1) / FT_THREADS, num_sms * 8));
+  k_cluster_tally<<<grid, FT_THREADS, 0, s>>>(in, st, nclust, rank, world, tl, map);
+  count_launch(1);
+}
 
 size_t final_tally_scan_words(int nclust) { return ((size_t)nclust + 1 + 1023) / 1024; }
 

@@ -156,6 +156,9 @@ size_t final_tally_scan_words(int nclust);
 void launch_final_tally(const DevIn &in, const DevState &st, const uint32_t *list, const unsigned long long *count, unsigned long long upper,
                         int nclust, int ncol, uint32_t *off, uint32_t *chk, uint32_t *cur, uint32_t *ord, uint32_t *scan_sums, int num_sms,
                         cudaStream_t s);
+// dd_final.cu: per-cluster tallies of the final output and $map over this rank's raws.  tl [5 * nclust] (abundance, n0, n1, nunq,
+// largest member reads) is zeroed by the caller; map [nraw] gets 0 for the raws of other ranks.
+void launch_cluster_tally(const DevIn &in, const DevState &st, int nclust, int rank, int world, uint32_t *tl, int32_t *map, int num_sms, cudaStream_t s);
 void launch_calc_pA_vec(const int *reads, const double *E, const int *prior, double *out, int n, cudaStream_t s);
 
 }  // namespace dd2
