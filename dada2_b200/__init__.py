@@ -3,7 +3,7 @@ reference's dada_uniques() interface.  See DESIGN.md / INTEGRATION.md."""
 from . import api  # noqa: F401
 from .api import Dada2bError, PackedCall, Resident, dada_uniques  # noqa: F401
 from . import bimera  # noqa: F401,E402
-from .bimera import removeBimeraDenovo  # noqa: F401,E402
+from .bimera import isShiftDenovo, removeBimeraDenovo  # noqa: F401,E402
 from . import merge  # noqa: F401,E402
 from . import derep  # noqa: F401,E402
 from . import errmodel  # noqa: F401,E402
@@ -22,3 +22,5 @@ from . import species  # noqa: F401,E402
 from .species import SpeciesDB, addSpecies, assignSpecies  # noqa: F401,E402
 from . import paired  # noqa: F401,E402
 from .paired import mergePairs  # noqa: F401,E402
+from . import align  # noqa: F401,E402
+from .align import nwalign  # noqa: F401,E402

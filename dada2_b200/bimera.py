@@ -330,3 +330,132 @@ def test_bimera_pairs(seqs, query, parent, allow_one_off=False, match=5, mismatc
 
 
 test_bimera_pairs.__test__ = False
+
+
+class ShiftOpts(C.Structure):
+    _fields_ = [("min_overlap", C.c_int32), ("match", C.c_int32), ("mismatch", C.c_int32), ("gap_p", C.c_int32)]
+
+
+class ShiftStats(C.Structure):
+    _fields_ = [("n_screened", C.c_int64), ("n_equal", C.c_int64), ("n_candidates", C.c_int64), ("n_filtered", C.c_int64),
+                ("n_aligned", C.c_int64), ("n_flagged", C.c_int64), ("n_cells", C.c_int64),
+                ("n_blocks", C.c_int64), ("gpu_launches", C.c_int64), ("ms_device", C.c_double), ("ms_k_align", C.c_double),
+                ("ms_total", C.c_double)]
+
+
+_SHIFT_BOUND = None       # the library object the argtypes were set on (a test may swap api's library)
+_ACGT_SET = frozenset("ACGT")
+
+
+def _shift_lib():
+    global _SHIFT_BOUND
+    L = api.lib()
+    if _SHIFT_BOUND is not L:
+        P = C.POINTER
+        L.dada2b_shift_default_opts.argtypes = [P(ShiftOpts)]
+        L.dada2b_shift_denovo.argtypes = [C.c_int32, C.c_char_p, C.c_void_p, C.c_void_p, P(ShiftOpts), C.c_int32, C.c_void_p,
+                                          P(ShiftStats), C.c_char_p]
+        L.dada2b_test_shift_pairs.argtypes = [C.c_int32, C.c_char_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, P(ShiftOpts),
+                                              C.c_int32, C.c_void_p, C.c_char_p]
+        _SHIFT_BOUND = L
+    return L
+
+
+def _shift_opts(minOverlap, match, mismatch, gap):
+    return ShiftOpts(int(minOverlap), int(match), int(mismatch), int(gap))
+
+
+def shift_flags(seqs, abunds, minOverlap=20, match=5, mismatch=-4, gap=-8, device=0, return_stats=False):
+    """The device call: distinct non-empty A/C/G/T sequences with their abundances -> uint8 flag[n] (isShiftDenovo's
+    shifts over them)."""
+    buf, off = _pack_seqs(seqs)
+    ab = np.ascontiguousarray(abunds, dtype=np.int64)
+    flag = np.zeros(len(seqs), np.uint8)
+    st = ShiftStats()
+    eb = C.create_string_buffer(ERRLEN)
+    o = _shift_opts(minOverlap, match, mismatch, gap)
+    rc = _shift_lib().dada2b_shift_denovo(len(seqs), buf, off.ctypes.data, ab.ctypes.data, C.byref(o), int(device), flag.ctypes.data,
+                                          C.byref(st), eb)
+    if rc:
+        raise api.Dada2bError(eb.value.decode())
+    if return_stats:
+        return flag, {k: getattr(st, k) for k, _ in ShiftStats._fields_}
+    return flag
+
+
+def test_shift_pairs(seqs, query, parent, minOverlap=20, match=5, mismatch=-4, gap=-8, device=0):
+    """Stage hook: -> int32[npairs, 5] = (prefix screen passes, overlap filter sends the pair to alignment, C_eval_pair's
+    match, mismatch, indel of nwalign(seqs[query[x]], seqs[parent[x]], band=-1)); the counts are always aligned."""
+    buf, off = _pack_seqs(seqs)
+    q = np.ascontiguousarray(query, dtype=np.int32)
+    p = np.ascontiguousarray(parent, dtype=np.int32)
+    if len(q) != len(p):
+        raise api.Dada2bError("dada2b: query and parent must have the same length.")
+    out = np.zeros((max(len(q), 1), 5), np.int32)
+    eb = C.create_string_buffer(ERRLEN)
+    o = _shift_opts(minOverlap, match, mismatch, gap)
+    rc = _shift_lib().dada2b_test_shift_pairs(len(seqs), buf, off.ctypes.data, len(q), q.ctypes.data, p.ctypes.data, C.byref(o),
+                                              int(device), out.ctypes.data, eb)
+    if rc:
+        raise api.Dada2bError(eb.value.decode())
+    return out[:len(q)]
+
+
+test_shift_pairs.__test__ = False
+
+
+def _shift_uniques(unqs):
+    """getUniques(unqs, silence=TRUE) and getSequences(unqs) for isShiftDenovo's input forms -> (dict, row sequences)."""
+    form = _form(unqs)
+    if form == "table":
+        mat, cols = np.asarray(unqs[0]), list(unqs[1])
+        cs = mat.sum(axis=0, dtype=np.int64)
+        tot = {}
+        for sq, a in zip(cols, cs):
+            tot[sq] = tot.get(sq, 0) + int(a)
+        return tot, cols
+    if form == "uniques":
+        seqs, ab = list(unqs.keys()), list(unqs.values())
+    elif form == "dada":
+        seqs, ab = list(unqs["denoised"].keys()), list(unqs["denoised"].values())
+    elif form == "derep":
+        seqs, ab = list(unqs["uniques"]), list(unqs["abundances"])
+    elif form == "merger":
+        seqs, ab = list(unqs["sequence"]), list(unqs["abundance"])
+    else:
+        raise ValueError(_UNRECOGNIZED)
+    tot = {}
+    for sq, a in zip(seqs, ab):                                     # a merger's duplicates are summed (getUniques' tapply)
+        tot[sq] = tot.get(sq, 0) + int(a)
+    return tot, seqs
+
+
+def isShiftDenovo(unqs, minOverlap=20, flagSubseqs=False, verbose=False, device=0):
+    """R/chimeras.R:384-400 on the GPU.  unqs: a {sequence: abundance} dict, a dada() result, a derep, a mergePairs merger
+    or a sequence table (mat, cols[, rows]) (its column sums).  -> bool[n]: whether each of getSequences(unqs), duplicates
+    included, is an exact shift (overlap >= minOverlap, not a containment) of a strictly more abundant unique.
+
+    flagSubseqs is accepted and has no effect, as in R (isShiftDenovo never passes it to isShift, :391).  An empty input
+    gives an empty array where R errors at seqs[shifts]."""
+    del flagSubseqs
+    tot, rows = _shift_uniques(unqs)
+    seqs = list(tot)
+    if not seqs:
+        return np.zeros(0, bool)
+    ab = np.array([tot[s] for s in seqs], np.int64)
+    if verbose:                                                     # :388-390, one line per sequence without parents
+        for a in ab:
+            if not np.any(ab > a):
+                print('[1] "No possible parents."')
+    # nwalign's C_isACGT error (R/misc.R:186-188) is reached by a sequence with a partner of different abundance
+    for s, a in zip(seqs, ab):
+        if not _ACGT_SET.issuperset(s) and np.any(ab != a):
+            raise api.Dada2bError("Sequences must contain only A/C/G/T characters.")
+    # "" is never flagged and flags nothing (match 0 is not < nchar("")); other letters are never reached past the check
+    dev = [k for k, s in enumerate(seqs) if s and _ACGT_SET.issuperset(s)]
+    shift = set()
+    if len(dev) > 1:
+        flag = shift_flags([seqs[k] for k in dev], ab[dev], minOverlap, device=device)
+        shift = {seqs[k] for k, f in zip(dev, flag) if f}
+    return np.array([s in shift for s in rows], bool)
+

@@ -14,10 +14,14 @@
 //   k_col_filter                thread per candidate: max over all shifts of the gapless ends-free score, and whether a
 //                               shift attaining it is an exact overlap; proves nwhamming > 0 for most candidates
 //   k_col_align                 warp per survivor: nw_warp (dd_nw_warp.cuh, unbanded or banded) + C_eval_pair (dd_evalpair.cuh)
+//
+// isShiftDenovo (include/dada2b_align.h; R/chimeras.R:384-415) runs the same screen and filter (DESIGN.md 24):
+//   k_shift_direct              drops screened pairs of equal abundance, directs the rest (less abundant = query)
+//   k_col_filter                with E restricted to the overlaps a shift can have
+//   k_nwalign                   (dd_align.cu) warp per survivor, unbanded ends-free, flags the query of every shift
 // Integer and bit work only.  There is no CPU fallback.
 #include "../../include/dada2b_collapse.h"
-#include "dd_evalpair.cuh"
-#include "dd_hostutil.h"
+#include "dd_align.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -166,15 +170,17 @@ __global__ void __launch_bounds__(256) k_col_allpairs(ColScreenArgs a) {
 struct ColFilterArgs {
   BimSeqs sq;
   int match, mismatch, unbanded;
+  int o_lo, o_trim;                         // E counts overlaps in [o_lo, min(l1, l2) - o_trim]: 1, 0 for collapse; max(m, 1), 1 for isShiftDenovo
   const int32_t *pq, *pr;                   // s1 = query, s2 = ref of each pair
   const unsigned long long *np_ptr;         // pair count (device)
   uint32_t *alist; unsigned long long *nalign;   // pairs that need alignment
   int32_t *verdict;                         // test hook: 1 = needs alignment (may be NULL)
 };
 
-// Exact overlap filter (DESIGN.md 17).  For every shift s (query base i against ref base i + s) with overlap o(s) > 0:
-// g(s) = match * m(s) + mismatch * x(s).  LB = max g, E = some shift attaining LB has x = 0.  Unbanded, LB > 0 and not E
-// prove nwhamming > 0.  Shifts go from the full-overlap plateau outwards, so o(s) only falls, and a shift whose best
+// Exact overlap filter (DESIGN.md 17, 24).  For every shift s (query base i against ref base i + s) with overlap o(s) > 0:
+// g(s) = match * m(s) + mismatch * x(s).  LB = max g, E = some shift attaining LB has x = 0 and o(s) in [o_lo, o_hi],
+// o_hi = min(l1, l2) - o_trim.
+// Unbanded, LB > 0 and not E prove nwhamming > 0 (collapse, [1, INT_MAX]) or that the pair is no shift (isShiftDenovo).  Shifts go from the full-overlap plateau outwards, so o(s) only falls, and a shift whose best
 // possible score o(s) * max(match, mismatch) is below LB can neither raise LB nor tie it exactly: the scan stops there.
 __global__ void __launch_bounds__(256) k_col_filter(ColFilterArgs a) {
   const unsigned long long np = *a.np_ptr;
@@ -201,8 +207,9 @@ __global__ void __launch_bounds__(256) k_col_filter(ColFilterArgs a) {
             mm += mism64(win64(rq, SW, lo + c, n), win64(rr, SW, lo + s + c, n));
           }
           const long long g = (long long)a.match * (o - mm) + (long long)a.mismatch * mm;
-          if (g > best) { best = g; exact = mm == 0; }
-          else if (g == best && mm == 0) exact = true;
+          const bool ex = mm == 0 && o >= a.o_lo && o <= min(l1, l2) - a.o_trim;
+          if (g > best) { best = g; exact = ex; }
+          else if (g == best && ex) exact = true;
           return true;
         };
         const int slo = min(0, l2 - l1), shi = max(0, l2 - l1);      // o(s) = min(l1, l2) on [slo, shi]
@@ -289,16 +296,7 @@ struct Ctx {
 };
 
 void check_opts(const dada2b_collapse_opts &o, const BimSeqs &sq) {
-  if (o.vec) {
-    // nwalign_vectorized2 keeps scores in int16.  Every cell of the ends-free matrix lies within A * minlen of 0, A =
-    // max(|match|, |mismatch|) (a diagonal path from the free first row or column reaches it), and a candidate adds one
-    // more score or gap: beyond 32767 the reference would wrap around, so such inputs are refused.
-    const long long A = std::max(std::llabs(o.match), std::llabs(o.mismatch));
-    const long long bound = A * sq.maxlen + std::max(A, std::llabs(o.gap_p));
-    if (bound > 32767 || std::llabs(o.gap_p) > 32767)
-      throw BErr{"dada2b: sequences too long for the vectorized aligner's 16-bit scores (max(|match|, |mismatch|) * maxlen + "
-                 "max(|match|, |mismatch|, |gap|) must stay <= 32767); use vec=FALSE."};
-  }
+  if (o.vec) check_int16(o.match, o.mismatch, o.gap_p, 1, sq.maxlen, 0);
 }
 
 // nw_warp's per-warp shared-memory layout and scratch, as in dd_merge.cu
@@ -313,21 +311,10 @@ void plan_align(ColAlignPlan &pl, const BimSeqs &sq, const dada2b_collapse_opts 
     const int m = std::min(std::min(o.mismatch, o.gap_p), std::min(o.match, 0));
     P.sentinel = (int)(int16_t)(INT16_MIN - m);                          // nwalign_vectorized.cpp:106
   } else P.sentinel = -9999;                                             // nwalign_endsfree.cpp:116-117
-  const int maxlen = sq.maxlen, minlen = sq.minlen;
-  const int lbmax = P.band < 0 ? maxlen : std::min(P.band + (maxlen - minlen), maxlen), rbmax = lbmax;
-  const int Wmax = lbmax + rbmax + 1;
-  const int nchunk = (((Wmax + 1) >> 1) + 31) >> 5;
+  const NwWarpLayout L = nw_warp_layout(sq.maxlen, sq.minlen, P.band);
   a.sq = sq;
-  a.seq_bytes = (maxlen + 15) & ~15;
-  a.H_words = (Wmax + 2 + 3) & ~3;
-  a.ops_words = ((2 * maxlen) / 16 + 2 + 3) & ~3;
-  a.mask_words = ((2 * maxlen + 31) / 32 + 2 + 3) & ~3;
-  a.ptr_words = (unsigned long long)(2 * maxlen + 2) * 2 * nchunk;
-  const int base_words = 2 * (a.seq_bytes / 4) + a.H_words + a.ops_words + 3 * a.mask_words;
-  a.ptr_in_smem = (4 * ((size_t)base_words + a.ptr_words) * 4 <= 96 * 1024) ? 1 : 0;
-  a.warp_words = base_words + (a.ptr_in_smem ? (int)a.ptr_words : 0);
-  pl.smem = (size_t)4 * a.warp_words * 4;
-  if (pl.smem > 200 * 1024) throw BErr{"dada2b: band/sequence length too large for the alignment kernel's shared memory."};
+  set_layout(a, L);
+  pl.smem = L.smem;
   BCK(cudaFuncSetAttribute(k_col_align, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(pl.smem, 48 * 1024)));
   pl.grid = num_sms * 8;
   if (!a.ptr_in_smem) {
@@ -379,6 +366,89 @@ void emit_block(Ctx &c, Screen &scr, const BimSeqs &sq, int m, int e0, int e1, i
   c.launches++;
 }
 
+// Blocks of producers whose pairs fit the budget (a single producer with more pairs gets a block of its own)
+void plan_blocks(const std::vector<int32_t> &cnt, std::vector<std::pair<int, int>> &blocks, unsigned long long &maxblk,
+                 unsigned long long &ncand) {
+  const int nseq = (int)cnt.size();
+  unsigned long long tot = 0;
+  for (int e = 0, b0 = 0; e < nseq; e++) {
+    if (tot && tot + (unsigned long long)cnt[e] > PAIR_BUDGET) { blocks.push_back({b0, e}); maxblk = std::max(maxblk, tot); b0 = e; tot = 0; }
+    tot += (unsigned long long)cnt[e]; ncand += (unsigned long long)cnt[e];
+    if (e == nseq - 1) { blocks.push_back({b0, nseq}); maxblk = std::max(maxblk, tot); }
+  }
+}
+
+// Test hooks: the screen over the whole set in one block -> every candidate {i < j} as (i << 32 | j), each exactly once
+std::unordered_set<unsigned long long> screen_set(Ctx &c, const BimSeqs &sq, int m, unsigned long long *d_ctr) {
+  std::unordered_set<unsigned long long> cand;
+  Screen scr;
+  std::vector<int32_t> cnt;
+  scr.build(c, sq, m);
+  scr.count(c, cnt);
+  unsigned long long want = 0;
+  for (int e = 0; e < sq.n; e++) want += (unsigned long long)cnt[e];
+  BBuf<int32_t> d_pr, d_pq;
+  d_pr.alloc(std::max(want, 1ull)); d_pq.alloc(std::max(want, 1ull));
+  emit_block(c, scr, sq, m, 0, sq.n, d_pr.p, d_pq.p, d_ctr + 4, want, d_ctr);
+  unsigned long long h[8];
+  std::vector<int32_t> pr(want), pq(want);
+  BCK(cudaMemcpyAsync(h, d_ctr, sizeof h, cudaMemcpyDeviceToHost, c.s));
+  if (want) {
+    BCK(cudaMemcpyAsync(pr.data(), d_pr.p, want * 4, cudaMemcpyDeviceToHost, c.s));
+    BCK(cudaMemcpyAsync(pq.data(), d_pq.p, want * 4, cudaMemcpyDeviceToHost, c.s));
+  }
+  BCK(cudaStreamSynchronize(c.s));
+  if (h[1] || h[4] != want) throw BErr{"dada2b: collapse screen produced a different number of pairs than it counted."};
+  for (unsigned long long t = 0; t < want; t++) {
+    if (!(pr[t] < pq[t])) throw BErr{"dada2b: collapse screen produced a pair out of order."};
+    if (!cand.insert((unsigned long long)pr[t] << 32 | (uint32_t)pq[t]).second) throw BErr{"dada2b: collapse screen produced a pair twice."};
+  }
+  return cand;
+}
+
+// isShiftDenovo: drops screened pairs of equal abundance (R compares strictly, R/chimeras.R:389) and directs the others
+// as (query = the less abundant, parent = the more abundant), compacted into dq / dp
+struct ShiftDirectArgs {
+  const int32_t *pr, *pq;
+  const unsigned long long *np_ptr;
+  const int64_t *ab;
+  int32_t *dq, *dp;
+  unsigned long long *ndir, *nequal;
+};
+
+__global__ void __launch_bounds__(256) k_shift_direct(ShiftDirectArgs a) {
+  const unsigned long long np = *a.np_ptr;
+  const int lane = threadIdx.x & 31;
+  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+  for (unsigned long long x0 = (unsigned long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); x0 < np; x0 += stride) {
+    const unsigned long long x = x0 + lane;
+    int i = 0, j = 0;
+    bool keep = false, eq = false;
+    if (x < np) {
+      i = a.pr[x]; j = a.pq[x];
+      const int64_t ai = a.ab[i], aj = a.ab[j];
+      eq = ai == aj;
+      keep = !eq;
+      if (ai > aj) { const int t = i; i = j; j = t; }                  // i: query (less abundant), j: parent
+    }
+    const unsigned b = __ballot_sync(0xffffffffu, keep), be = __ballot_sync(0xffffffffu, eq);
+    unsigned long long base = 0;
+    if (lane == 0) {
+      if (b) base = atomicAdd(a.ndir, (unsigned long long)__popc(b));
+      if (be) atomicAdd(a.nequal, (unsigned long long)__popc(be));
+    }
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (keep) { const unsigned long long t = base + __popc(b & lanemask_lt()); a.dq[t] = i; a.dp[t] = j; }
+  }
+}
+
+dada2b_nwalign_opts shift_align_opts(const dada2b_shift_opts &o) {   // isShiftedPair: nwalign(sq, par, band=-1), :407
+  dada2b_nwalign_opts n;
+  dada2b_nwalign_default_opts(&n);
+  n.match = o.match; n.mismatch = o.mismatch; n.gap_p = o.gap_p; n.homo_gap_p = o.gap_p;
+  return n;
+}
+
 }  // namespace
 
 }  // namespace dd2
@@ -419,19 +489,14 @@ int dada2b_collapse_nomismatch(int32_t nseq, const char *seq_concat, const int64
     std::vector<int32_t> cnt;
     if (m >= 1) { scr.build(c, sq, m); scr.count(c, cnt); }
     else { cnt.resize(nseq); for (int e = 0; e < nseq; e++) cnt[e] = e; }
-    // blocks of producers whose pairs fit the budget (a single producer with more pairs gets a block of its own)
     std::vector<std::pair<int, int>> blocks;
-    unsigned long long maxblk = 1, tot = 0, ncand = 0;
-    for (int e = 0, b0 = 0; e < nseq; e++) {
-      if (tot && tot + (unsigned long long)cnt[e] > PAIR_BUDGET) { blocks.push_back({b0, e}); maxblk = std::max(maxblk, tot); b0 = e; tot = 0; }
-      tot += (unsigned long long)cnt[e]; ncand += (unsigned long long)cnt[e];
-      if (e == nseq - 1) { blocks.push_back({b0, nseq}); maxblk = std::max(maxblk, tot); }
-    }
+    unsigned long long maxblk = 1, ncand = 0;
+    plan_blocks(cnt, blocks, maxblk, ncand);
     BBuf<int32_t> d_pr, d_pq, d_zq, d_zr; BBuf<uint32_t> d_alist; BBuf<unsigned long long> d_ctr;
     d_pr.alloc(maxblk); d_pq.alloc(maxblk); d_alist.alloc(maxblk); d_zq.alloc(maxblk); d_zr.alloc(maxblk); d_ctr.alloc(8);
     // d_ctr: [0] cells, [1] overflow, [2] error, [4] pairs, [5] aligned, [6] zero
     BCK(cudaMemsetAsync(d_ctr.p, 0, 64, c.s));
-    ColFilterArgs fa{sq, opts->match, opts->mismatch, opts->band < 0 ? 1 : 0, d_pq.p, d_pr.p, d_ctr.p + 4, d_alist.p, d_ctr.p + 5, nullptr};
+    ColFilterArgs fa{sq, opts->match, opts->mismatch, opts->band < 0 ? 1 : 0, 1, 0, d_pq.p, d_pr.p, d_ctr.p + 4, d_alist.p, d_ctr.p + 5, nullptr};
     ColAlignArgs &aa = pl.a;
     aa.pq = d_pq.p; aa.pr = d_pr.p; aa.alist = d_alist.p; aa.nalign = d_ctr.p + 5; aa.ham = nullptr;
     aa.zq = d_zq.p; aa.zr = d_zr.p; aa.nzero = d_ctr.p + 6; aa.ctr = d_ctr.p;
@@ -526,30 +591,7 @@ int dada2b_test_collapse_pairs(int32_t nseq, const char *seq_concat, const int64
     BCK(cudaMemsetAsync(d_ctr.p, 0, 64, c.s));
     // 1. the product's screen over the whole set, in one block: the candidate set, each unordered pair exactly once
     std::unordered_set<unsigned long long> cand;
-    if (m >= 1) {
-      Screen scr;
-      std::vector<int32_t> cnt;
-      scr.build(c, sq, m);
-      scr.count(c, cnt);
-      unsigned long long want = 0;
-      for (int e = 0; e < nseq; e++) want += (unsigned long long)cnt[e];
-      BBuf<int32_t> d_pr, d_pq;
-      d_pr.alloc(std::max(want, 1ull)); d_pq.alloc(std::max(want, 1ull));
-      emit_block(c, scr, sq, m, 0, nseq, d_pr.p, d_pq.p, d_ctr.p + 4, want, d_ctr.p);
-      unsigned long long h[8];
-      std::vector<int32_t> pr(want), pq(want);
-      BCK(cudaMemcpyAsync(h, d_ctr.p, sizeof h, cudaMemcpyDeviceToHost, c.s));
-      if (want) {
-        BCK(cudaMemcpyAsync(pr.data(), d_pr.p, want * 4, cudaMemcpyDeviceToHost, c.s));
-        BCK(cudaMemcpyAsync(pq.data(), d_pq.p, want * 4, cudaMemcpyDeviceToHost, c.s));
-      }
-      BCK(cudaStreamSynchronize(c.s));
-      if (h[1] || h[4] != want) throw BErr{"dada2b: collapse screen produced a different number of pairs than it counted."};
-      for (unsigned long long t = 0; t < want; t++) {
-        if (!(pr[t] < pq[t])) throw BErr{"dada2b: collapse screen produced a pair out of order."};
-        if (!cand.insert((unsigned long long)pr[t] << 32 | (uint32_t)pq[t]).second) throw BErr{"dada2b: collapse screen produced a pair twice."};
-      }
-    }
+    if (m >= 1) cand = screen_set(c, sq, m, d_ctr.p);
     for (int x = 0; x < npairs; x++) {
       const int a = std::min(query[x], ref[x]), b = std::max(query[x], ref[x]);
       out3[3 * (size_t)x] = m < 1 ? (a != b) : (int)cand.count((unsigned long long)a << 32 | (uint32_t)b);
@@ -562,7 +604,7 @@ int dada2b_test_collapse_pairs(int32_t nseq, const char *seq_concat, const int64
       BCK(cudaMemcpyAsync(d_r.p, ref, (size_t)npairs * 4, cudaMemcpyHostToDevice, c.s));
       const unsigned long long np = (unsigned long long)npairs;
       BCK(cudaMemcpyAsync(d_ctr.p + 4, &np, 8, cudaMemcpyHostToDevice, c.s));
-      ColFilterArgs fa{sq, opts->match, opts->mismatch, opts->band < 0 ? 1 : 0, d_q.p, d_r.p, d_ctr.p + 4, nullptr, nullptr, d_ver.p};
+      ColFilterArgs fa{sq, opts->match, opts->mismatch, opts->band < 0 ? 1 : 0, 1, 0, d_q.p, d_r.p, d_ctr.p + 4, nullptr, nullptr, d_ver.p};
       k_col_filter<<<std::max(1, std::min(c.num_sms * 16, (npairs + 255) / 256)), 256, 0, c.s>>>(fa);
       ColAlignPlan pl;
       plan_align(pl, sq, *opts, c.num_sms);
@@ -578,6 +620,167 @@ int dada2b_test_collapse_pairs(int32_t nseq, const char *seq_concat, const int64
       BCK(cudaGetLastError());
       if (h[2]) throw BErr{"N-W Align out of range."};
       for (int x = 0; x < npairs; x++) { out3[3 * (size_t)x + 1] = ver[x]; out3[3 * (size_t)x + 2] = ham[x]; }
+    }
+  } catch (BErr &e) { msg = e.msg; rc = 1; }
+  catch (std::exception &e) { msg = e.what(); rc = 1; }
+  if (rc && errbuf) snprintf(errbuf, DADA2B_ERRLEN, "%s", msg.c_str());
+  return rc;
+}
+
+void dada2b_shift_default_opts(dada2b_shift_opts *o) {          // R/chimeras.R:384 + getDadaOpt defaults
+  o->min_overlap = 20; o->match = 5; o->mismatch = -4; o->gap_p = -8;
+}
+
+// isShiftDenovo (R/chimeras.R:384-400): every pair the screen passes, of different abundances, directed, filtered, aligned
+int dada2b_shift_denovo(int32_t nseq, const char *seq_concat, const int64_t *seq_off, const int64_t *abund,
+                        const dada2b_shift_opts *opts, int32_t device, uint8_t *flag, dada2b_shift_stats *stats,
+                        char errbuf[DADA2B_ERRLEN]) {
+  const double t0 = bnow_ms();
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr, ka = nullptr, kb = nullptr;
+  int rc = 0;
+  std::string msg;
+  try {
+    if (!opts || !flag || !abund) throw BErr{"dada2b: NULL argument."};
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) throw BErr{"dada2b: no CUDA device available (this library has no CPU path)."};
+    BCK(cudaSetDevice(device));
+    Ctx c;
+    BCK(cudaDeviceGetAttribute(&c.num_sms, cudaDevAttrMultiProcessorCount, device));
+    BCK(cudaStreamCreateWithFlags(&c.s, cudaStreamNonBlocking));
+    BCK(cudaEventCreate(&ev0)); BCK(cudaEventCreate(&ev1)); BCK(cudaEventCreate(&ka)); BCK(cudaEventCreate(&kb));
+    BCK(cudaEventRecord(ev0, c.s));
+    long long h2d = 0;
+    BimSeqs sq{};
+    BBuf<uint32_t> d_seq2; BBuf<uint16_t> d_len; std::vector<uint16_t> len;
+    upload_packed_seqs(nseq, seq_concat, seq_off, c.s, d_seq2, d_len, len, sq, h2d, "isShiftDenovo");
+    const int m = opts->min_overlap;
+    NwAlignPlan pl;
+    nwalign_plan(pl, sq, shift_align_opts(*opts), c.num_sms);
+    Screen scr;
+    std::vector<int32_t> cnt;
+    if (m >= 1) { scr.build(c, sq, m); scr.count(c, cnt); }
+    else { cnt.resize(nseq); for (int e = 0; e < nseq; e++) cnt[e] = e; }
+    std::vector<std::pair<int, int>> blocks;
+    unsigned long long maxblk = 1, nscreen = 0;
+    plan_blocks(cnt, blocks, maxblk, nscreen);
+    BBuf<int32_t> d_pr, d_pq, d_dq, d_dp; BBuf<uint32_t> d_alist; BBuf<unsigned long long> d_ctr; BBuf<int64_t> d_ab; BBuf<uint8_t> d_flag;
+    d_pr.alloc(maxblk); d_pq.alloc(maxblk); d_dq.alloc(maxblk); d_dp.alloc(maxblk); d_alist.alloc(maxblk); d_ctr.alloc(8);
+    d_ab.alloc(nseq); d_flag.alloc(nseq);
+    BCK(cudaMemcpyAsync(d_ab.p, abund, (size_t)nseq * 8, cudaMemcpyHostToDevice, c.s));
+    BCK(cudaMemsetAsync(d_flag.p, 0, (size_t)nseq, c.s));
+    // d_ctr: [0] cells, [1] overflow, [2] error, [4] pairs, [5] aligned, [6] directed, [7] equal
+    BCK(cudaMemsetAsync(d_ctr.p, 0, 64, c.s));
+    const ShiftDirectArgs da{d_pr.p, d_pq.p, d_ctr.p + 4, d_ab.p, d_dq.p, d_dp.p, d_ctr.p + 6, d_ctr.p + 7};
+    // the filter's E counts the overlaps a shift can have: match in [max(m, 1), min(l1, l2) - 1] (:409-410)
+    const ColFilterArgs fa{sq, opts->match, opts->mismatch, 1, std::max(m, 1), 1, d_dq.p, d_dp.p, d_ctr.p + 6, d_alist.p, d_ctr.p + 5, nullptr};
+    NwAlignArgs &aa = pl.a;
+    aa.s1 = d_dq.p; aa.s2 = d_dp.p; aa.alist = d_alist.p; aa.npairs_ptr = d_ctr.p + 5; aa.flag = d_flag.p; aa.min_overlap = m;
+    aa.ctr = d_ctr.p;
+    unsigned long long naligned = 0, nequal = 0, ncand = 0;
+    for (auto &b : blocks) {
+      unsigned long long want = 0;
+      for (int e = b.first; e < b.second; e++) want += (unsigned long long)cnt[e];
+      if (!want) continue;
+      BCK(cudaMemsetAsync(d_ctr.p + 4, 0, 32, c.s));
+      emit_block(c, scr, sq, m, b.first, b.second, d_pr.p, d_pq.p, d_ctr.p + 4, want, d_ctr.p);
+      const int g = (int)std::max<unsigned long long>(1, std::min<unsigned long long>((unsigned long long)c.num_sms * 16, (want + 255) / 256));
+      k_shift_direct<<<g, 256, 0, c.s>>>(da);
+      k_col_filter<<<g, 256, 0, c.s>>>(fa);
+      BCK(cudaEventRecord(ka, c.s));
+      nwalign_launch(pl, c.s);
+      BCK(cudaEventRecord(kb, c.s));
+      c.launches += 4;
+      unsigned long long h[8];
+      BCK(cudaMemcpyAsync(h, d_ctr.p, sizeof h, cudaMemcpyDeviceToHost, c.s));
+      BCK(cudaStreamSynchronize(c.s));
+      BCK(cudaGetLastError());
+      if (h[1] || h[4] != want) throw BErr{"dada2b: collapse screen produced a different number of pairs than it counted."};
+      if (h[2]) throw BErr{"N-W Align out of range."};                                   // nwalign_endsfree.cpp:184
+      float ms = 0;
+      BCK(cudaEventElapsedTime(&ms, ka, kb)); c.ms_align += ms;
+      naligned += h[5]; ncand += h[6]; nequal += h[7];
+    }
+    BCK(cudaMemcpyAsync(flag, d_flag.p, (size_t)nseq, cudaMemcpyDeviceToHost, c.s));
+    unsigned long long h[8];
+    BCK(cudaMemcpyAsync(h, d_ctr.p, sizeof h, cudaMemcpyDeviceToHost, c.s));
+    BCK(cudaEventRecord(ev1, c.s));
+    BCK(cudaStreamSynchronize(c.s));
+    if (stats) {
+      memset(stats, 0, sizeof *stats);
+      stats->n_screened = (int64_t)nscreen; stats->n_equal = (int64_t)nequal; stats->n_candidates = (int64_t)ncand;
+      stats->n_aligned = (int64_t)naligned; stats->n_filtered = (int64_t)(ncand - naligned);
+      int64_t nf = 0;
+      for (int i = 0; i < nseq; i++) nf += flag[i] != 0;
+      stats->n_flagged = nf; stats->n_cells = (int64_t)h[0]; stats->n_blocks = (int64_t)blocks.size();
+      stats->gpu_launches = c.launches;
+      float ms = 0;
+      BCK(cudaEventElapsedTime(&ms, ev0, ev1)); stats->ms_device = ms;
+      stats->ms_k_align = c.ms_align;
+      stats->ms_total = bnow_ms() - t0;
+    }
+  } catch (BErr &e) { msg = e.msg; rc = 1; }
+  catch (std::exception &e) { msg = e.what(); rc = 1; }
+  for (cudaEvent_t e : {ev0, ev1, ka, kb}) if (e) cudaEventDestroy(e);
+  if (rc && errbuf) snprintf(errbuf, DADA2B_ERRLEN, "%s", msg.c_str());
+  return rc;
+}
+
+int dada2b_test_shift_pairs(int32_t nseq, const char *seq_concat, const int64_t *seq_off, int32_t npairs, const int32_t *query,
+                            const int32_t *parent, const dada2b_shift_opts *opts, int32_t device, int32_t *out5,
+                            char errbuf[DADA2B_ERRLEN]) {
+  int rc = 0;
+  std::string msg;
+  try {
+    if (!opts || (npairs && (!query || !parent || !out5))) throw BErr{"dada2b: NULL argument."};
+    if (npairs < 0) throw BErr{"dada2b: negative pair count."};
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) throw BErr{"dada2b: no CUDA device available (this library has no CPU path)."};
+    BCK(cudaSetDevice(device));
+    Ctx c;
+    BCK(cudaDeviceGetAttribute(&c.num_sms, cudaDevAttrMultiProcessorCount, device));
+    BCK(cudaStreamCreateWithFlags(&c.s, cudaStreamNonBlocking));
+    long long h2d = 0;
+    BimSeqs sq{};
+    BBuf<uint32_t> d_seq2; BBuf<uint16_t> d_len; std::vector<uint16_t> len;
+    upload_packed_seqs(nseq, seq_concat, seq_off, c.s, d_seq2, d_len, len, sq, h2d, "isShiftDenovo");
+    for (int x = 0; x < npairs; x++)
+      if (query[x] < 0 || query[x] >= nseq || parent[x] < 0 || parent[x] >= nseq) throw BErr{"dada2b: bad pair index."};
+    const int m = opts->min_overlap;
+    BBuf<unsigned long long> d_ctr;
+    d_ctr.alloc(8);
+    BCK(cudaMemsetAsync(d_ctr.p, 0, 64, c.s));
+    std::unordered_set<unsigned long long> cand;
+    if (m >= 1) cand = screen_set(c, sq, m, d_ctr.p);
+    for (int x = 0; x < npairs; x++) {
+      const int a = std::min(query[x], parent[x]), b = std::max(query[x], parent[x]);
+      out5[5 * (size_t)x] = m < 1 ? (a != b) : (int)cand.count((unsigned long long)a << 32 | (uint32_t)b);
+    }
+    if (npairs) {
+      BBuf<int32_t> d_q, d_p, d_ver, d_cnt;
+      d_q.alloc(npairs); d_p.alloc(npairs); d_ver.alloc(npairs); d_cnt.alloc(3 * (size_t)npairs);
+      BCK(cudaMemcpyAsync(d_q.p, query, (size_t)npairs * 4, cudaMemcpyHostToDevice, c.s));
+      BCK(cudaMemcpyAsync(d_p.p, parent, (size_t)npairs * 4, cudaMemcpyHostToDevice, c.s));
+      const unsigned long long np = (unsigned long long)npairs;
+      BCK(cudaMemcpyAsync(d_ctr.p + 4, &np, 8, cudaMemcpyHostToDevice, c.s));
+      const ColFilterArgs fa{sq, opts->match, opts->mismatch, 1, std::max(m, 1), 1, d_q.p, d_p.p, d_ctr.p + 4, nullptr, nullptr, d_ver.p};
+      k_col_filter<<<std::max(1, std::min(c.num_sms * 16, (npairs + 255) / 256)), 256, 0, c.s>>>(fa);
+      NwAlignPlan pl;
+      nwalign_plan(pl, sq, shift_align_opts(*opts), c.num_sms);
+      NwAlignArgs &aa = pl.a;
+      aa.s1 = d_q.p; aa.s2 = d_p.p; aa.npairs = np; aa.counts = d_cnt.p; aa.ctr = d_ctr.p;
+      nwalign_launch(pl, c.s);
+      std::vector<int32_t> ver(npairs), cn(3 * (size_t)npairs);
+      unsigned long long h[8];
+      BCK(cudaMemcpyAsync(ver.data(), d_ver.p, (size_t)npairs * 4, cudaMemcpyDeviceToHost, c.s));
+      BCK(cudaMemcpyAsync(cn.data(), d_cnt.p, (size_t)npairs * 12, cudaMemcpyDeviceToHost, c.s));
+      BCK(cudaMemcpyAsync(h, d_ctr.p, sizeof h, cudaMemcpyDeviceToHost, c.s));
+      BCK(cudaStreamSynchronize(c.s));
+      BCK(cudaGetLastError());
+      if (h[2]) throw BErr{"N-W Align out of range."};
+      for (int x = 0; x < npairs; x++) {
+        int32_t *o = out5 + 5 * (size_t)x;
+        o[1] = ver[x]; o[2] = cn[3 * (size_t)x]; o[3] = cn[3 * (size_t)x + 1]; o[4] = cn[3 * (size_t)x + 2];
+      }
     }
   } catch (BErr &e) { msg = e.msg; rc = 1; }
   catch (std::exception &e) { msg = e.what(); rc = 1; }

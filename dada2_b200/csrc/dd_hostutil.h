@@ -1,6 +1,7 @@
 // Host-side helpers shared by the drivers of dd_bimera.cu and dd_merge.cu (product code).
 #pragma once
 #include "dd_bimera.cuh"
+#include <algorithm>
 #include <chrono>
 #include <climits>
 #include <string>
@@ -57,6 +58,40 @@ inline void upload_packed_seqs(int nseq, const char *seq_concat, const int64_t *
   BCK(cudaStreamSynchronize(s));                 // `packed` is pageable and goes out of scope
   h2d += (long long)packed.size() * 4 + (long long)nseq * 2;
   sq.seq2 = d_seq2.p; sq.len = d_len.p;
+}
+
+// Per-warp shared-memory layout of a warp-per-pair nw_warp kernel (k_merge_pairs, k_col_align, k_nwalign): the two
+// unpacked rows, the diagonal scores H, the move string, three column masks for eval_pair_warp and, when it fits in 96 KB
+// per block of four warps, the move matrix; otherwise that goes to a global scratch row per warp.  All sizes in 32-bit
+// words except seq_bytes and smem.
+struct NwWarpLayout {
+  int warp_words, seq_bytes, H_words, ops_words, mask_words, ptr_in_smem;
+  unsigned long long ptr_words;
+  size_t smem;                                   // dynamic shared memory of a 128-thread block
+};
+
+inline NwWarpLayout nw_warp_layout(int maxlen, int minlen, int band) {
+  NwWarpLayout L;
+  const int lbmax = band < 0 ? maxlen : std::min(band + (maxlen - minlen), maxlen), rbmax = lbmax;
+  const int Wmax = lbmax + rbmax + 1;
+  const int nchunk = (((Wmax + 1) >> 1) + 31) >> 5;
+  L.seq_bytes = (maxlen + 15) & ~15;
+  L.H_words = (Wmax + 2 + 3) & ~3;
+  L.ops_words = ((2 * maxlen) / 16 + 2 + 3) & ~3;
+  L.mask_words = ((2 * maxlen + 31) / 32 + 2 + 3) & ~3;
+  L.ptr_words = (unsigned long long)(2 * maxlen + 2) * 2 * nchunk;
+  const int base_words = 2 * (L.seq_bytes / 4) + L.H_words + L.ops_words + 3 * L.mask_words;
+  L.ptr_in_smem = (4 * ((size_t)base_words + L.ptr_words) * 4 <= 96 * 1024) ? 1 : 0;
+  L.warp_words = base_words + (L.ptr_in_smem ? (int)L.ptr_words : 0);
+  L.smem = (size_t)4 * L.warp_words * 4;
+  if (L.smem > 200 * 1024) throw BErr{"dada2b: band/sequence length too large for the alignment kernel's shared memory."};
+  return L;
+}
+
+// Copies the layout into a kernel's argument struct (fields of the same names).
+template <typename A> inline void set_layout(A &a, const NwWarpLayout &L) {
+  a.warp_words = L.warp_words; a.seq_bytes = L.seq_bytes; a.H_words = L.H_words; a.ops_words = L.ops_words;
+  a.mask_words = L.mask_words; a.ptr_in_smem = L.ptr_in_smem; a.ptr_words = L.ptr_words;
 }
 
 }  // namespace dd2

@@ -84,25 +84,14 @@ void merge_setup(const BimSeqs &sq, const dada2b_merge_opts *opts, int num_sms, 
   P.match = opts->match; P.mismatch = opts->mismatch; P.gap = opts->gap_p; P.hgap = opts->homo_gap_p; P.band = opts->band;
   P.homo = opts->gap_p != opts->homo_gap_p ? 1 : 0;                     // evaluate.cpp:40-46
   P.sentinel = -9999;                                                    // nwalign_endsfree.cpp:116-117
-  const int maxlen = sq.maxlen, minlen = sq.minlen;
-  const int lbmax = P.band < 0 ? maxlen : std::min(P.band + (maxlen - minlen), maxlen), rbmax = lbmax;
-  const int Wmax = lbmax + rbmax + 1;
-  const int nchunk = (((Wmax + 1) >> 1) + 31) >> 5;
+  const NwWarpLayout L = nw_warp_layout(sq.maxlen, sq.minlen, P.band);
   a.sq = sq;
-  a.seq_bytes = (maxlen + 15) & ~15;
-  a.H_words = (Wmax + 2 + 3) & ~3;
-  a.ops_words = ((2 * maxlen) / 16 + 2 + 3) & ~3;
-  a.mask_words = ((2 * maxlen + 31) / 32 + 2 + 3) & ~3;
-  a.ptr_words = (unsigned long long)(2 * maxlen + 2) * 2 * nchunk;
-  const int base_words = 2 * (a.seq_bytes / 4) + a.H_words + a.ops_words + 3 * a.mask_words;
-  a.ptr_in_smem = (4 * ((size_t)base_words + a.ptr_words) * 4 <= 96 * 1024) ? 1 : 0;
-  a.warp_words = base_words + (a.ptr_in_smem ? (int)a.ptr_words : 0);
-  smem = (size_t)4 * a.warp_words * 4;
-  if (smem > 200 * 1024) throw BErr{"dada2b: band/sequence length too large for the alignment kernel's shared memory."};
+  set_layout(a, L);
+  smem = L.smem;
   BCK(cudaFuncSetAttribute(k_merge_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
   grid = (int)std::min<long long>((long long)num_sms * 8, std::max<long long>(1, ((long long)npairs + 3) / 4));
   if (!a.ptr_in_smem) { d_ptr.alloc((size_t)grid * 4 * a.ptr_words); a.ptr_scratch = d_ptr.p; }
-  a.trim_overhang = opts->trim_overhang != 0; a.npairs = npairs; a.cons_stride = 2 * maxlen;
+  a.trim_overhang = opts->trim_overhang != 0; a.npairs = npairs; a.cons_stride = 2 * sq.maxlen;
 }
 
 }  // namespace dd2

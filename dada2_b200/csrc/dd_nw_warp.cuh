@@ -46,6 +46,11 @@ __device__ __forceinline__ int step_dlo(int k, int len1, const BandGeom &g) {
 // s1/s2: bytes, bits 1:0 = base, bit 2 = "inside a homopolymer run >= 3".  H: W+2 ints.
 // ptr: 2*nchunk words per step, (len1+len2+1) steps.  Returns number of ops; ops (1 diag, 2 gap in
 // centre row, 3 gap in raw row) are packed 2 bits each into opw in traceback (reverse) order.
+// GLOBAL: nwalign() of nwalign_endsfree.cpp:403-537 (endsfree=FALSE): row 0 and column 0 hold cumulative gap penalties
+// (:417-427) and the last row and column pay for their gaps.  With a band, the reference overwrites (lband+1, 0) and
+// (0, rband+1) with -9999 (:446-447); those are the cells of diagonals -lb-1 and rb+1, which keep the sentinel here.
+// Homopolymer costs do not apply (evaluate.cpp:49-52).
+template <bool GLOBAL = false>
 __device__ inline int nw_warp(const uint8_t *s1, int len1, const uint8_t *s2, int len2, const AlnParams &P, int *H,
                        uint32_t *ptr, uint32_t *opw, unsigned long long *cells, int *err) {
   const int lane = lane_id();
@@ -69,15 +74,15 @@ __device__ inline int nw_warp(const uint8_t *s1, int len1, const uint8_t *s2, in
         const int i = (k - dl) >> 1, j = (k + dl) >> 1;
         int *h = H + dl + g.lb + 1;
         int val;
-        if (i == 0) { val = 0; p = 2; }                 // nwalign_endsfree.cpp:97-101
-        else if (j == 0) { val = 0; p = 3; }            // :91-95
+        if (i == 0) { val = GLOBAL ? j * P.gap : 0; p = 2; }     // nwalign_endsfree.cpp:97-101
+        else if (j == 0) { val = GLOBAL ? i * P.gap : 0; p = 3; } // :91-95
         else {
           const int c1 = s1[i - 1], c2 = s2[j - 1];
           int left, up, diag;
-          if (i == len1) left = h[-1];                                   // :130-137 (homo :303-311)
-          else left = h[-1] + ((P.homo && (c2 & 4)) ? P.hgap : P.gap);
-          if (j == len2) up = h[1];                                      // :139-144 (homo :313-320)
-          else up = h[1] + ((P.homo && (c1 & 4)) ? P.hgap : P.gap);
+          if (!GLOBAL && i == len1) left = h[-1];                        // :130-137 (homo :303-311)
+          else left = h[-1] + ((!GLOBAL && P.homo && (c2 & 4)) ? P.hgap : P.gap);
+          if (!GLOBAL && j == len2) up = h[1];                           // :139-144 (homo :313-320)
+          else up = h[1] + ((!GLOBAL && P.homo && (c1 & 4)) ? P.hgap : P.gap);
           diag = h[0] + (((c1 ^ c2) & 3) ? P.mismatch : P.match);
           if (up >= diag && up >= left) { val = up; p = 3; }             // :147-156
           else if (left >= diag) { val = left; p = 2; }

@@ -1,5 +1,5 @@
 """Sequence tables: makeSequenceTable and collapseNoMismatch (R/multiSample.R:31-55, :104-160), plus nwhamming
-(R/misc.R:216-220) batched over pairs.
+(R/misc.R:216-220) batched over pairs on the public aligner (align.py).
 
 collapseNoMismatch's double loop over the table's columns (:125-144) runs in libdada2b.so behind
 include/dada2b_collapse.h: the prefix screen, the exact overlap filter and the alignments on the GPU, the greedy order on
@@ -13,7 +13,7 @@ import sys
 
 import numpy as np
 
-from . import api
+from . import align, api
 from .bimera import _pack_seqs
 
 ERRLEN = 256
@@ -88,20 +88,14 @@ def test_collapse_pairs(seqs, query, ref, minOverlap=20, vec=True, band=-1, matc
 test_collapse_pairs.__test__ = False
 
 
-def nwhamming(s1, s2, vec=False, band=-1, match=5, mismatch=-4, gap=-8, device=0):
+def nwhamming(s1, s2, vec=False, band=-1, match=5, mismatch=-4, gap=-8, homo_gap=None, endsfree=True, device=0):
     """R/misc.R:216-220 (nwalign, then C_eval_pair's mismatch + indel), vectorised over pairs like R's Vectorize:
-    strings or equal-length lists of strings.  -> int, or int32 array for lists."""
-    one = isinstance(s1, str) and isinstance(s2, str)
-    a = [s1] if isinstance(s1, str) else list(s1)
-    b = [s2] if isinstance(s2, str) else list(s2)
-    if len(a) == 1 and len(b) > 1:
-        a = a * len(b)
-    if len(b) == 1 and len(a) > 1:
-        b = b * len(a)
-    if len(a) != len(b):
-        raise api.Dada2bError("dada2b: nwhamming needs pairs of sequences.")
-    out = test_collapse_pairs(a + b, np.arange(len(a)), np.arange(len(a), 2 * len(a)), minOverlap=0, vec=vec, band=band, match=match,
-                              mismatch=mismatch, gap=gap, device=device)[:, 2]
+    strings or equal-length lists of strings; the keyword arguments are nwalign's (R's `...`).  -> int, or int32 array
+    for lists."""
+    a, b, one = align._pairs(s1, s2, "nwhamming")
+    cnt = align.eval_counts(a, b, device=device, match=match, mismatch=mismatch, gap=gap, homo_gap=homo_gap, band=band,
+                            endsfree=endsfree, vec=vec)
+    out = cnt[:, 1] + cnt[:, 2]
     return int(out[0]) if one else out
 
 
