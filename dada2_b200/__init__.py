@@ -24,3 +24,5 @@ from . import paired  # noqa: F401,E402
 from .paired import mergePairs  # noqa: F401,E402
 from . import align  # noqa: F401,E402
 from .align import nwalign  # noqa: F401,E402
+from . import qc  # noqa: F401,E402
+from .qc import plotComplexity, plotQualityProfile  # noqa: F401,E402

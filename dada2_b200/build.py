@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdada2b.so")
-SOURCES = ["dd_kernels.cu", "dd_final.cu", "dd_nwfwd.cu", "dd_nwrow.cu", "dd_nwlane.cu", "dd_prescreen.cu", "dd_round.cu", "dd_round2.cu", "dd_driver.cu", "dd_bimera.cu", "dd_bimfwd.cu", "dd_bimfwd16.cu", "dd_merge.cu", "dd_pairs.cu", "dd_derep.cu", "dd_collapse.cu", "dd_align.cu", "dd_filter.cu", "dd_primer.cu", "dd_pool.cu", "dd_taxonomy.cu", "dd_species.cu"]
+SOURCES = ["dd_kernels.cu", "dd_final.cu", "dd_nwfwd.cu", "dd_nwrow.cu", "dd_nwlane.cu", "dd_prescreen.cu", "dd_round.cu", "dd_round2.cu", "dd_driver.cu", "dd_bimera.cu", "dd_bimfwd.cu", "dd_bimfwd16.cu", "dd_merge.cu", "dd_pairs.cu", "dd_derep.cu", "dd_collapse.cu", "dd_align.cu", "dd_filter.cu", "dd_primer.cu", "dd_pool.cu", "dd_taxonomy.cu", "dd_species.cu", "dd_qprofile.cu"]
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-fmad=false",
          "-Xcompiler", "-fPIC,-O2,-pthread", "-diag-suppress", "550"]
 
@@ -15,7 +15,7 @@ def needs_build():
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(os.path.dirname(HERE), "include", f) for f in ("dada2b.h", "dada2b_test.h", "dada2b_bimera.h", "dada2b_merge.h", "dada2b_derep.h", "dada2b_collapse.h", "dada2b_align.h", "dada2b_filter.h", "dada2b_primer.h", "dada2b_pool.h", "dada2b_taxonomy.h", "dada2b_species.h")]
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(os.path.dirname(HERE), "include", f) for f in ("dada2b.h", "dada2b_test.h", "dada2b_bimera.h", "dada2b_merge.h", "dada2b_derep.h", "dada2b_collapse.h", "dada2b_align.h", "dada2b_filter.h", "dada2b_primer.h", "dada2b_pool.h", "dada2b_taxonomy.h", "dada2b_species.h", "dada2b_qprofile.h")]
     deps.append(os.path.abspath(__file__))          # FLAGS (target architecture) live here: a library built with other flags is stale
     return any(os.path.getmtime(d) > t for d in deps)
 
