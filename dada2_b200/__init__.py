@@ -8,6 +8,7 @@ from . import merge  # noqa: F401,E402
 from . import derep  # noqa: F401,E402
 from . import errmodel  # noqa: F401,E402
 from . import seqtab  # noqa: F401,E402
+from .seqtab import mergeSequenceTables  # noqa: F401,E402
 from . import filter  # noqa: F401,E402
 from .filter import filterAndTrim, filter_reads  # noqa: F401,E402
 from . import primer  # noqa: F401,E402
